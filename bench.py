@@ -1,7 +1,8 @@
 # -*- coding: utf-8 -*-
-"""bench.py -- accepted tokens/sec of the LOOKAHEAD draft-verify loop (BASELINE.json metric) on B200.
+"""bench.py -- accepted tokens/sec of the LOOKAHEAD draft-verify loop (BASELINE.json metric) on an H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--model llama2-7b|...]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A "step" is one request through the hot path: a 256-token synthetic prompt -> greedy generation of 256 new tokens
@@ -12,7 +13,9 @@ constructed so that greedy decoding is a noisy first-order chain over the vocabu
 random layers' context-dependent contribution flips the arg-max).  Such text re-uses n-grams across requests like
 real text does, so a trie warmed on OTHER prompts (the reference's warm-up, benchmarks/benchmark.py:159-169)
 yields accepted lengths > 1 on prompts it has never seen - the headline is that first pass, not answer replay.
-One JSON line is printed by rank 0; see README.md / DESIGN.md 5 for the keys.  N > 1 = independent data-parallel
+One JSON line is printed by rank 0; see README.md / DESIGN.md 5 for the keys.  --dump-outputs DIR writes what the
+last timed step returned to its caller (generated token ids, accepted draft lengths) as float64 .npy files, so that
+two builds can be compared output for output: prompts and weights are seeded, identical from run to run.  N > 1 = independent data-parallel
 replicas (the loop is per request, pretrained_model.py:1152): one NCCL broadcast of the weights, then no collective on
 the data path; every replica runs the same K requests (identical work per rank, weak scaling).
 """
@@ -33,10 +36,12 @@ MODELS = {
     # name: (family, hidden, inter, layers, heads, kv_heads, vocab, repetition_penalty of its BASELINE config)
     'llama2-7b': ('llama', 4096, 11008, 32, 32, 32, 32000, 1.0),
     'mistral-7b': ('mistral', 4096, 14336, 32, 32, 8, 32000, 1.1),
-    'mixtral-8x7b': ('mixtral', 4096, 14336, 32, 32, 8, 32000, 1.0),
+    # Mixtral-8x7B's layer shape, 16 of its 32 layers: all 32 are ~93 GB of bf16 weights, more than one 80 GB H100 holds;
+    # 16 layers (~47 GB) leave room for the KV cache and keep the per-layer verify work (attention + 8 experts) intact
+    'mixtral-8x7b-16l': ('mixtral', 4096, 14336, 16, 32, 8, 32000, 1.0),
     'tiny': ('llama', 512, 1024, 4, 4, 4, 32000, 1.0),
 }
-METRIC_NAMES = {'llama2-7b': 'Llama-2-7B', 'mistral-7b': 'Mistral-7B', 'mixtral-8x7b': 'Mixtral-8x7B', 'tiny': 'tiny'}
+METRIC_NAMES = {'llama2-7b': 'Llama-2-7B', 'mistral-7b': 'Mistral-7B', 'mixtral-8x7b-16l': 'Mixtral-8x7B (16 of 32 layers)', 'tiny': 'tiny'}
 PROMPT_LEN, NEW_TOKENS, DL, BL = 256, 256, 64, 8
 EMBED_STD = float(os.environ.get("PIA_BENCH_EMBED_STD", "5.5"))   # signal of the successor chain vs the layers' noise
 LM_SCALE = 0.25
@@ -152,11 +157,12 @@ def synth_fill(model, cfg, seed=0, embed_std=None):
 
 
 class ClockSampler(threading.Thread):
-    """SM clock + throttle reasons during the timed region (B200_PROFILING.md clocks line), via NVML"""
+    """GPU name, power limit, SM clock + throttle reasons during the timed region, via NVML"""
 
     def __init__(self, index):
         super().__init__(daemon=True)
         self.index, self.samples, self.reasons, self.stop_flag, self.max_mhz = index, [], set(), False, None
+        self.gpu, self.power_limit_w = None, None
 
     def run(self):
         try:
@@ -164,6 +170,9 @@ class ClockSampler(threading.Thread):
             nv.nvmlInit()
             h = nv.nvmlDeviceGetHandleByIndex(self.index)
             self.max_mhz = nv.nvmlDeviceGetMaxClockInfo(h, nv.NVML_CLOCK_SM)
+            self.gpu = nv.nvmlDeviceGetName(h)
+            self.gpu = self.gpu.decode() if isinstance(self.gpu, bytes) else self.gpu
+            self.power_limit_w = nv.nvmlDeviceGetPowerManagementLimit(h) / 1000.0
             names = {nv.nvmlClocksThrottleReasonHwSlowdown: 'hw_slowdown',
                      nv.nvmlClocksThrottleReasonHwThermalSlowdown: 'hw_thermal_slowdown',
                      nv.nvmlClocksThrottleReasonSwThermalSlowdown: 'sw_thermal_slowdown',
@@ -181,18 +190,19 @@ class ClockSampler(threading.Thread):
 
     def summary(self):
         s = sorted(self.samples)
-        return {'sm_mhz': s[len(s) // 2] if s else None, 'sm_max_mhz': self.max_mhz, 'reasons': sorted(self.reasons)}
+        return {'gpu': self.gpu, 'power_limit_w': self.power_limit_w, 'sm_mhz': s[len(s) // 2] if s else None,
+                'sm_max_mhz': self.max_mhz, 'reasons': sorted(self.reasons)}
 
 
 def peaks():
-    """(HBM GB/s, dense bf16 TFLOP/s, source): the pool's measured numbers (MEASURED_PEAKS.json, driver-written) or the
-    fallback B200_PROFILING.md states"""
+    """(HBM GB/s, dense bf16 TFLOP/s, source): measured numbers from MEASURED_PEAKS.json when present, else the H100
+    SXM data sheet (3.35 TB/s HBM3, 989 dense bf16 TFLOP/s at 700 W; not reached)"""
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     try:
         d = json.load(open(p))
-        return float(d['hbm_gbs']), float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 1400.0))), 'measured'
+        return float(d['hbm_gbs']), float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 989.0))), 'measured'
     except (OSError, ValueError, KeyError, TypeError):
-        return 6650.0, 1400.0, 'fallback'
+        return 3350.0, 989.0, 'fallback'
 
 
 def timed_requests(K, rank=0):
@@ -253,6 +263,7 @@ def run_ours(args):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         barrier()
         e0.record()
+        o = None
         for x in ins:
             o = model.generate(input_ids=x.to(dev, non_blocking=True) if host_io else x, **gen)
             seq = o.sequences.cpu() if host_io else o.sequences
@@ -277,7 +288,7 @@ def run_ours(args):
         else:
             s_e, n_e = float(sum(edls)), float(len(edls))
         return dict(ms=ms, tokens=toks, mean_edl=s_e / max(n_e, 1), steps=n_e, launches=int(launches), outs=outs,
-                    per_rank_ms=per_rank)
+                    per_rank_ms=per_rank, last=o)
 
     trie = model.lookahead_cache
     snap = trie.snapshot()              # the trie after the disjoint warm-up: both timed passes start from it
@@ -297,6 +308,8 @@ def run_ours(args):
         dist.all_gather(allc, t)
         per_rank_clocks = [{'sm_mhz': int(c[0]), 'sm_max_mhz': int(c[1]), 'n_throttle_reasons': int(c[2])} for c in allc]
     same_tokens = all(torch.equal(a.cpu(), b.cpu()) for a, b in zip(res['outs'], e2e['outs']))
+    if rank == 0 and args.dump_outputs and res['last'] is not None:
+        dump_outputs(args.dump_outputs, res['last'].sequences.cpu().numpy(), res['last'].kwargs['edls'])
     extra = {}
     if rank == 0:
         extra['roofline'] = gemm_roofline(model, dev)
@@ -346,6 +359,14 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, sequences, edls):
+    """what the last timed request returned to its caller: the token ids [1, prompt + generated] and the accepted length
+    of each verify step, float64 (token ids are exact), a few KB in all"""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, 'sequences.npy'), np.asarray(sequences, dtype=np.float64).reshape(1, -1))
+    np.save(os.path.join(out_dir, 'accepted_lengths.npy'), np.asarray(edls, dtype=np.float64))
+
+
 def workload_config(args, world, peaks_src):
     penalty = MODELS[args.model][7]
     return {'workload': f'{args.model} bf16, greedy, {DL}-token/{BL}-branch trie draft, {PROMPT_LEN}-token prompt -> '
@@ -369,12 +390,12 @@ def weight_bytes_per_step(model):
     return n
 
 
-def ncu_traffic(prefix, kernel):
-    """DRAM bytes (read + written) per launch of `kernel` from the newest committed `ncu --set full` summary whose
-    capture name starts with `prefix` (profiles/*_traffic.json, written by scripts/summarize_profiles.py); None when
-    there is no such capture"""
+def ncu_traffic(prefix, kernel, profiles_dir=os.path.join(ROOT, 'profiles')):
+    """DRAM bytes (read + written) per launch of `kernel` from the newest `ncu --set full` summary whose capture name
+    starts with `prefix` (profiles/*_traffic.json, written by scripts/summarize_profiles.py); None when there is no
+    such capture"""
     import glob
-    for f in sorted(glob.glob(os.path.join(ROOT, 'profiles', '*_traffic.json')), reverse=True):
+    for f in sorted(glob.glob(os.path.join(profiles_dir, '*_traffic.json')), reverse=True):
         try:
             for k, v in json.load(open(f)).items():
                 name, _, kern = k.partition(':')
@@ -405,7 +426,7 @@ def _graph_time(fn, reps=20):
 
 
 def gemm_roofline(model, dev):
-    """the step's dominant kernel by the committed launch list (profiles/*_launches.md): k_gemm_ws on the fused
+    """the step's largest weight stream: k_gemm_ws on the fused
     gate/up projection.  All layers' plans in turn (their weights together exceed L2, so every launch streams cold
     HBM), CUDA events around graph replays; algorithmic bytes = the weight once + the 64 activation rows + the output"""
     rt = model._rt
@@ -774,7 +795,10 @@ def run_reference(args):
     allp = phrase_bank_prompts(64 + 8 * max(Wm, 1), cfg.vocab_size)
     for i in range(Wm):
         cpu_request(model, trie, allp[64 + i % (8 * max(Wm, 1))], penalty)
-    samples = [cpu_request(model, trie, allp[j], penalty) for j in timed_requests(K)]
+    timed = timed_requests(K)
+    samples = [cpu_request(model, trie, allp[j], penalty) for j in timed]
+    if args.dump_outputs and samples:
+        dump_outputs(args.dump_outputs, allp[timed[-1]] + samples[-1]['tokens'], samples[-1]['edls'])
     toks = sum(len(s['tokens']) for s in samples)
     secs = sum(s['seconds'] for s in samples)
     edls = [e for s in samples for e in s['edls'][1:]]
@@ -807,6 +831,8 @@ if __name__ == '__main__':
     ap.add_argument('--model', default='llama2-7b', choices=sorted(MODELS))
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-batched', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step as DIR/<name>.npy')
     a = ap.parse_args()
     if a.impl == 'reference':
         run_reference(a)

@@ -1,5 +1,5 @@
 /*
- * pia_b200.h -- C ABI of libpia_b200.so: the B200 (sm_100a) draft -> verify -> accept hot loop of
+ * pia_b200.h -- C ABI of libpia_b200.so: the H100 (sm_90a) draft -> verify -> accept hot loop of
  * PIA LOOKAHEAD.
  *
  * The reference path has no FFI: it is plain Python (SURVEY.md 8b).  This ABI therefore sits *below* the
@@ -226,7 +226,7 @@ int pia_tree_attn_fused_fwd(pia_attn_plan_t *p, int layer, const void *d_qkv, co
 /* ============================================================================================
  * Weight-streaming GEMM of the verify forward: Y[t, n] = sum_k X[t, k] W[n, k]  (X: <= 64 draft rows, W = an
  * nn.Linear weight [N, K] bf16), i.e. the projections of modeling_llama.py:254-256, :303, :185-186, :769.
- * TMA + tcgen05, weights read once; see csrc/gemm_ws.cu.
+ * TMA + wgmma, weights read once; see csrc/gemm_ws.cu.
  * ============================================================================================ */
 typedef struct pia_gemm_plan pia_gemm_plan_t;
 /* d_x : [x_rows >= 64, K] bf16 activation buffer the plan's TMA descriptor is bound to; K % 64 == 0.

@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""B200-native (sm_100a) draft -> verify -> accept hot loop of PIA LOOKAHEAD behind the reference's Python surface.
+"""H100-native (sm_90a) draft -> verify -> accept hot loop of PIA LOOKAHEAD behind the reference's Python surface.
 
     from painlessinferenceacceleration_b200.common.lookahead_cache import LookaheadCache, Tree
     from painlessinferenceacceleration_b200.models.llama.modeling_llama import LlamaForCausalLM

@@ -28,7 +28,7 @@ class _DeviceTrie(object):
     def __init__(self, device, eos_ids, stop_words, max_node, max_output_node, vocab_capacity, node_capacity,
                  edge_capacity, n_input_slots, max_put_tokens, frontier_capacity, max_resident_queries):
         if not torch.cuda.is_available():
-            raise RuntimeError('LookaheadCache needs a CUDA device (B200); there is no CPU fallback')
+            raise RuntimeError('LookaheadCache needs a CUDA device (H100); there is no CPU fallback')
         self.lib = L.load()
         self.device = torch.device(device if device is not None else f'cuda:{torch.cuda.current_device()}')
         cfg = L.TrieConfig(vocab_capacity, node_capacity, edge_capacity, n_input_slots, max_node, max_output_node,

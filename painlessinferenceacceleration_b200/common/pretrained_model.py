@@ -2,7 +2,7 @@
 """LookaheadPreTrainedModel: the reference's generation surface
 (/root/reference/lookahead/lookahead/common/pretrained_model.py: class :48, generate :108, lookahead_prepare_inputs
 :666-756, _lookahead_update_model_kwargs :764-892, _update_cache :894-945, lookahead_generation :947-1268,
-stream_generate :1323-1350) re-built B200-first.
+stream_generate :1323-1350) re-built H100-first.
 
 The reference loop crosses the host/device boundary several times per step (draft ids + n x n mask H2D, one argmax
 + .tolist() sync per accepted token, kv_idx H2D, a torch.cat of the whole KV cache per layer).  Here one decode step

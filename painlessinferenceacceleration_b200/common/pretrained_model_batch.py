@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""Batched LOOKAHEAD loop, B200-native: the reference's
+"""Batched LOOKAHEAD loop, H100-native: the reference's
 /root/reference/lookahead/lookahead/common/pretrained_model_batch.py (lookahead_prepare_inputs_for_generation
 :664-759 with LookaheadCache.bat_get lookahead_cache.py:519-561, _lookahead_update_model_kwargs_for_generation
 :767-935, _early_stop :937-980, _update_cache :982-989, lookahead_generation :1002-1330) and the cursor-addressed

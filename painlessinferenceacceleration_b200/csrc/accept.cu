@@ -1,4 +1,4 @@
-// Longest-prefix accept, sequence update and KV compaction of the LOOKAHEAD loop (sm_100a).
+// Longest-prefix accept, sequence update and KV compaction of the LOOKAHEAD loop (sm_90a).
 //
 // Takes over common/pretrained_model.py:764-892 (_lookahead_update_model_kwargs_for_generation) and :894-945
 // (_update_cache*).  The reference walks the draft on the host with one GPU arg-max plus one .tolist() sync per

@@ -1,4 +1,4 @@
-// Shared host/device helpers of libpia_b200.so (sm_100a only).
+// Shared host/device helpers of libpia_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,7 +47,7 @@ constexpr unsigned FULL = 0xffffffffu;
 // Programmatic dependent launch (PDL): every kernel of the decode step is launched with the
 // programmatic-stream-serialization attribute, announces its dependents at once and waits for its predecessor
 // (griddepcontrol.wait = predecessor complete + memory visible) before its first global access.  The next kernel's
-// CTAs are then resident, with barriers/TMEM set up, when the predecessor's last CTA retires, which hides the
+// CTAs are then resident, with barriers set up, when the predecessor's last CTA retires, which hides the
 // launch + prologue latency between the ~330 small kernels of a step.  PIA_PDL=0 disables the attribute (the
 // device-side instructions are no-ops for a normally launched kernel).
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

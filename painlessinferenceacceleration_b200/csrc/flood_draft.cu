@@ -1,4 +1,4 @@
-// FLOOD's hash-table lookahead draft behind its `Spec` interface (sm_100a) -- SURVEY.md 8f-4.
+// FLOOD's hash-table lookahead draft behind its `Spec` interface (sm_90a) -- SURVEY.md 8f-4.
 //
 // Takes over the Triton kernels of /root/reference/flood/flood/ops/draft.py that flood/utils/speculative.py's
 // `Lookahead(Spec)` (:23-124) calls:

@@ -1,4 +1,4 @@
-// Elementwise pieces of the LOOKAHEAD verify forward (sm_100a), all HBM-bound, 16-byte vectorised:
+// Elementwise pieces of the LOOKAHEAD verify forward (sm_90a), all HBM-bound, 16-byte vectorised:
 //   k_rmsnorm           models/llama/modeling_llama.py:76-90   (+ the residual add of the decoder layer :340-352)
 //   k_rope_kv_append    :156-169 apply_rotary_pos_emb at the tree positions of :587, and the KV-cache append
 //                       that replaces the reference's per-step torch.cat (:265-268)

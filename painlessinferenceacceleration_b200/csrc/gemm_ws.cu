@@ -1,17 +1,17 @@
-// Weight-streaming GEMM for the verify forward (sm_100a: TMA + tcgen05 + TMEM).
+// Weight-streaming GEMM for the verify forward (sm_90a: TMA + wgmma).
 //
 //   Y[t, n] = sum_k X[t, k] * W[n, k]        X: [TOK <= 64 draft rows, K] bf16,  W: [N, K] bf16 (nn.Linear weight)
 //
 // i.e. the q/k/v/o/gate/up/down/lm_head projections of the reference's patched forward
 // (models/llama/modeling_llama.py:254-256, :303, :185-186, :769) at the draft's row count.  With <= 64 rows the
 // GEMM is a pure weight stream (arithmetic intensity = rows FLOP/B << ridge), so the kernel is built around HBM:
-//   * swap-AB: 128 weight rows are the UMMA M dimension, the 64 tokens the UMMA N dimension; D[128 x 64] fp32 lives in
-//     64 TMEM columns, so the big operand (W) is read exactly once and only the small one (X, <= 1.4 MB, L2 resident)
-//     is re-read per tile;
-//   * one CTA per (128-row weight tile, K split): warp 0 = TMA producer over a 4-stage mbarrier ring of
-//     {W tile 128x64 (16 KB), X tile 64x64 (8 KB)} SWIZZLE_128B boxes, warp 1 = single-thread tcgen05.mma issuer
-//     (4 x UMMA 128x64x16 per stage), warps 2-5 = epilogue (tcgen05.ld -> bf16 / fp32 store).  ~100 KB of shared
-//     memory per CTA so that two CTAs share an SM and one CTA's prologue/epilogue hides behind the other's stream;
+//   * swap-AB: 128 weight rows are the MMA M dimension (two warpgroups x wgmma M = 64), the 64 tokens the N
+//     dimension; the fp32 accumulator D[128 x 64] lives in registers (32 per thread), so the big operand (W) is read
+//     exactly once and only the small one (X, <= 1.4 MB, L2 resident) is re-read per tile;
+//   * one CTA per (128-row weight tile, K split): warps 0-7 = two consumer warpgroups (wgmma.m64n64k16, both operands
+//     from shared memory, then the epilogue), warp 8 = TMA producer over an mbarrier ring of {W tile 128x64 (16 KB),
+//     X tile 64x64 (8 KB)} SWIZZLE_128B boxes.  ~100 KB of shared memory per CTA so that two CTAs share an SM and
+//     one CTA's prologue/epilogue hides behind the other's stream;
 //   * projections with few weight tiles (o_proj, down_proj: N = 4096 -> 32 tiles) split K across CTAs and write fp32
 //     partial slices that the consumer (k_rmsnorm_partials) sums in a fixed order - deterministic, no atomics.
 #include <cuda.h>
@@ -24,18 +24,25 @@
 namespace pia {
 namespace gemm {
 
-constexpr int BMW = 128;   // weight rows per tile (UMMA M)
+constexpr int BMW = 128;   // weight rows per tile (two wgmma M = 64 halves)
 constexpr int BK = 64;     // k elements per stage (one 128-byte swizzle row)
-constexpr int TOK = 64;    // token rows (UMMA N)
-constexpr int NTHREADS = 192;
+constexpr int TOK = 64;    // token rows (wgmma N)
+constexpr int NTHREADS = 288;  // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int PRODUCER_WARP = 8;
 constexpr int W_BYTES = BMW * BK * 2, X_BYTES = TOK * BK * 2, STAGE_BYTES = W_BYTES + X_BYTES;
 constexpr int XCH_BYTES = TOK * 64 * 2;  // bf16 [64 tokens][64 rows] exchange tile of the SiLU*up epilogue
 constexpr int smem_total(int nstage) { return nstage * STAGE_BYTES + 256 + XCH_BYTES + 1024; }
-constexpr int TMEM_COLS = 64;
+// the accumulator tile [128 rows][64 tokens] fp32 is staged through the (dead) pipeline stages after the main loop, one
+// row per epilogue thread; it starts past the 32 KB that the cluster split-K reduction receives from its peers
+constexpr int ACC_OFF = 32 * 1024, ACC_LD = TOK + 4;
+static_assert(ACC_OFF + BMW * ACC_LD * 4 <= 4 * STAGE_BYTES, "accumulator staging must fit in the pipeline stages");
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -75,44 +82,50 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t addr, uint32_t *v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(addr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// K-major SWIZZLE_128B operand descriptor (cute::UMMA::SmemDescriptor): 8-row groups 1024 B apart
+// K-major SWIZZLE_128B wgmma operand descriptor (sm_90 GMMA descriptor): 8-row groups 1024 B apart
 __device__ __forceinline__ uint64_t kmajor_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;           // LBO (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32; // SBO
-  d |= (uint64_t)1 << 46;           // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;           // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;           // SWIZZLE_128B
   return d;
 }
-// bf16 x bf16 -> fp32, M = 128, N = TOK, both operands K-major
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TOK >> 3) << 17) | ((uint32_t)(BMW >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// the accumulator registers are written asynchronously: this pins every read of them after the wait above
+__device__ __forceinline__ void fence_acc(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 64] += A[64 x 16] * B[64 x 16]^T, bf16 in, fp32 accumulate, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b)
+      : "memory");
+}
+// one stage (BK = 64 k) of this warpgroup's 64 weight rows against the 64 tokens
+__device__ __forceinline__ void mma_stage(float (&acc)[32], uint32_t wa, uint32_t xa) {
+  wgmma_fence();
+#pragma unroll
+  for (int j = 0; j < BK / 16; ++j) wgmma_m64n64k16(acc, kmajor_desc(wa + j * 32), kmajor_desc(xa + j * 32));
+  wgmma_commit();
+  wgmma_wait_all();
+  fence_acc(acc);
+}
+// accumulator fragment element -> (row of the warpgroup's 64, token): register 4*i + 2*h + e holds
+// row 16 * (warp % 4) + lane / 4 + 8 * h, token 8 * i + 2 * (lane % 4) + e
+__device__ __forceinline__ int frag_row(int warp, int lane, int h) { return 16 * (warp & 3) + (lane >> 2) + 8 * h; }
+__device__ __forceinline__ int frag_tok(int lane, int i) { return 8 * i + 2 * (lane & 3); }
 
 struct Params {
   int N, K, n_split, chunks_per_split, n_chunks, rows, tiled;
@@ -128,7 +141,7 @@ struct Params {
 
 // NSTAGE = 4: ~100 KB of shared memory, two CTAs per SM (grids with more CTAs than SMs);
 // NSTAGE = 8: ~200 KB, one CTA per SM with twice the bytes in flight (grids that do not fill the SMs twice) -
-// HBM only saturates with >= ~10 MB of loads in flight chip-wide.
+// HBM only saturates with several MB of loads in flight chip-wide.
 template <int NSTAGE>
 __global__ void __launch_bounds__(NTHREADS, NSTAGE <= 4 ? 2 : 1)
 k_gemm_ws(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, Params p) {
@@ -137,8 +150,7 @@ k_gemm_ws(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t bar_full = base + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE, bar_acc = bar_empty + 8 * NSTAGE;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(sm + SMEM_BAR + 16 * NSTAGE + 16);
+  const uint32_t bar_full = base + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE;
   // grid = (tiles, splits), or (splits, tiles) when the splits of a tile form a cluster (clusters run along x)
   const int tile = p.cluster ? blockIdx.y : blockIdx.x, split = p.cluster ? blockIdx.x : blockIdx.y;
   const int n0 = tile * BMW;
@@ -150,25 +162,18 @@ k_gemm_ws(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
   const int nch = c1 - c0;
 
   if (tid == 0) {
-    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-    mbar_init(bar_acc, 1);
+    // a stage is free again once each of the 8 consumer warps has seen its wgmma on it complete
+    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncwarp();  // warp 0 reconverges before the block barrier below
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (!p.no_pdl) pdl_launch_dependents();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  // Barriers + TMEM are set up while the previous kernel drains, and - the weights being immutable - the first
-  // NSTAGE weight tiles are already streaming from HBM before griddepcontrol.wait: only the activation tiles (and
-  // the output stores) depend on the predecessor, so its run time hides this kernel's pipeline fill.
+  // Barriers are set up while the previous kernel drains, and - the weights being immutable - the first NSTAGE weight
+  // tiles are already streaming from HBM before griddepcontrol.wait: only the activation tiles (and the output
+  // stores) depend on the predecessor, so its run time hides this kernel's pipeline fill.
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       auto load_w = [&](int i, int s) {
         const uint32_t wd = base + s * STAGE_BYTES;
@@ -192,136 +197,142 @@ k_gemm_ws(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
     }
     __syncwarp();
     if (p.cluster) { cluster_sync_all(); cluster_sync_all(); }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < nch; ++i) {
-        const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
-        mbar_wait(bar_full + 8 * s, ph);
-        tc_fence_after();
-        const uint32_t wa = base + s * STAGE_BYTES, xa = wa + W_BYTES;
+    return;
+  }
+
+  // ---------------------------------------------------------------- consumers: warpgroup wg owns weight rows [64 wg, +64)
+  pdl_wait();  // output stores (and the WAR hazard on the output buffer) are ordered after the predecessor
+  const int wg = warp >> 2;
+  float acc[32];
 #pragma unroll
-        for (int j = 0; j < BK / 16; ++j)
-          umma_bf16(tmem, kmajor_desc(wa + j * 32), kmajor_desc(xa + j * 32), IDESC, (i | j) != 0);
-        umma_commit(bar_empty + 8 * s);
-      }
-      umma_commit(bar_acc);
-    }
+  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+  for (int i = 0; i < nch; ++i) {
+    const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
+    mbar_wait(bar_full + 8 * s, ph);
+    const uint32_t wa = base + s * STAGE_BYTES, xa = wa + W_BYTES;
+    mma_stage(acc, wa + wg * 64 * 128, xa);
     __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+  }
+  // stage the tile through shared memory so that the epilogue thread of weight row r holds its 64 tokens
+  float *accs = reinterpret_cast<float *>(sm + ACC_OFF);
+  asm volatile("bar.sync 2, 256;" ::: "memory");  // every wgmma of both warpgroups has read its last stage
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = wg * 64 + frag_row(warp, lane, h);
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<float2 *>(accs + r * ACC_LD + frag_tok(lane, i)) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+  }
+  asm volatile("bar.sync 2, 256;" ::: "memory");
+  if (wg == 1) {
     if (p.cluster) { cluster_sync_all(); cluster_sync_all(); }
-  } else {
-    // epilogue: thread = one weight row n (TMEM lane), 64 token values in registers
-    pdl_wait();  // output stores (and the WAR hazard on the output buffer) are ordered after the predecessor
-    const int q = warp & 3;
-    const int n = n0 + q * 32 + lane;
-    uint32_t v[64];
-    if (nch > 0) {
-      mbar_wait(bar_acc, 0);
-      tc_fence_after();
-      const uint32_t a = tmem + ((uint32_t)(q * 32) << 16);
-      tmem_ld32(a, v);
-      tmem_ld32(a + 32, v + 32);
-      tmem_ld_wait();
+    return;
+  }
+
+  // epilogue (warps 0-3): thread = one weight row n, 64 token values in registers
+  const int q = warp;
+  const int n = n0 + q * 32 + lane;
+  uint32_t v[64];
+  {
+    const float4 *src = reinterpret_cast<const float4 *>(accs + (q * 32 + lane) * ACC_LD);
+#pragma unroll
+    for (int t = 0; t < 16; ++t) {
+      const float4 a = src[t];
+      v[4 * t] = __float_as_uint(a.x); v[4 * t + 1] = __float_as_uint(a.y);
+      v[4 * t + 2] = __float_as_uint(a.z); v[4 * t + 3] = __float_as_uint(a.w);
+    }
+  }
+  if (p.cluster) {
+    // split-K inside a cluster: after everyone has left its main loop (barrier A: the pipeline stages of every CTA
+    // are dead) each thread pushes its fp32 row - 16 token quads, quad-major so that the lanes of a warp write
+    // consecutive 16-byte words - into the CTA that owns that row slice, barrier B, and the owner adds the
+    // cluster's partials in split order (deterministic) and writes bf16.  No fp32 round trip through HBM/L2.
+    const int cs = p.cluster, RS = BMW / cs;      // rows per owner CTA: 64 (2 splits) or 32 (4 splits)
+    cluster_sync_all();
+    {
+      const int row = q * 32 + lane;
+      const int owner = row / RS, rl = row % RS;
+      const uint32_t dst = map_to_cta(base + (uint32_t)((split * 16) * RS + rl) * 16, owner);
+#pragma unroll
+      for (int tq = 0; tq < 16; ++tq)
+        st_cluster_f4(dst + (uint32_t)(tq * RS) * 16, __uint_as_float(v[4 * tq]), __uint_as_float(v[4 * tq + 1]),
+                      __uint_as_float(v[4 * tq + 2]), __uint_as_float(v[4 * tq + 3]));
+    }
+    cluster_sync_all();
+    {
+      const int e = warp * 32 + lane;             // 0..127
+      const int rl = e % RS, tg = e / RS;         // row of this CTA's slice, token group
+      const int qpt = RS / 8;                     // token quads per thread: 16 / (128 / RS)
+      const int n_out = n0 + split * RS + rl;     // this CTA's rank in the cluster == its split index
+      const float4 *buf = reinterpret_cast<const float4 *>(sm);
+      __nv_bfloat16 *ob = p.out_bf16 + grp * p.out_group_stride;
+      if (n_out < p.N) {
+        for (int tq = tg * qpt; tq < (tg + 1) * qpt; ++tq) {
+          float4 a = buf[(0 * 16 + tq) * RS + rl];
+          for (int src = 1; src < cs; ++src) {
+            const float4 b = buf[(src * 16 + tq) * RS + rl];
+            a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+          }
+          const int t0 = 4 * tq;
+          if (t0 < p.rows) ob[(long long)t0 * p.N + n_out] = __float2bfloat16_rn(a.x);
+          if (t0 + 1 < p.rows) ob[(long long)(t0 + 1) * p.N + n_out] = __float2bfloat16_rn(a.y);
+          if (t0 + 2 < p.rows) ob[(long long)(t0 + 2) * p.N + n_out] = __float2bfloat16_rn(a.z);
+          if (t0 + 3 < p.rows) ob[(long long)(t0 + 3) * p.N + n_out] = __float2bfloat16_rn(a.w);
+        }
+      }
+    }
+  } else
+  if (p.silu) {
+    // act(gate) * up (modeling_llama.py:185-186) in the epilogue: rows 0-63 (warps q = 0, 1) hold gate rows, rows
+    // 64-127 (q = 2, 3) the up rows of the same 64 output columns.  Each warp pair splits the 64 tokens: the gate warp
+    // finishes tokens 0-31 (it receives the up values through shared memory), the up warp tokens 32-63 (it receives the
+    // gate values), so all four warps share the exponentials.  Rounding points as in eager bf16 (and k_silu_mul):
+    // GEMM out -> bf16, silu -> bf16, product -> bf16.
+    __nv_bfloat16 *xu = reinterpret_cast<__nv_bfloat16 *>(sm + SMEM_BAR + 256);  // up   [32 tokens 0-31 ][64 rows]
+    __nv_bfloat16 *xg = xu + 32 * 64;                                             // gate [32 tokens 32-63][64 rows]
+    const int rr = (q & 1) * 32 + lane;
+    if (q >= 2) {
+#pragma unroll
+      for (int t = 0; t < 32; ++t) xu[t * 64 + rr] = __float2bfloat16_rn(__uint_as_float(v[t]));
     } else {
 #pragma unroll
-      for (int t = 0; t < 64; ++t) v[t] = 0u;
+      for (int t = 0; t < 32; ++t) xg[t * 64 + rr] = __float2bfloat16_rn(__uint_as_float(v[32 + t]));
     }
-    if (p.cluster) {
-      // split-K inside a cluster: after everyone has left its main loop (barrier A: the pipeline stages of every CTA
-      // are dead) each thread pushes its fp32 row - 16 token quads, quad-major so that the lanes of a warp write
-      // consecutive 16-byte words - into the CTA that owns that row slice, barrier B, and the owner adds the
-      // cluster's partials in split order (deterministic) and writes bf16.  No fp32 round trip through HBM/L2.
-      const int cs = p.cluster, RS = BMW / cs;      // rows per owner CTA: 64 (2 splits) or 32 (4 splits)
-      cluster_sync_all();
-      {
-        const int row = q * 32 + lane;
-        const int owner = row / RS, rl = row % RS;
-        const uint32_t dst = map_to_cta(base + (uint32_t)((split * 16) * RS + rl) * 16, owner);
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    const int col = tile * 64 + rr;
+    const int inter = p.N >> 1;
+    if (col < inter) {
+      const int tb = q < 2 ? 0 : 32;
 #pragma unroll
-        for (int tq = 0; tq < 16; ++tq)
-          st_cluster_f4(dst + (uint32_t)(tq * RS) * 16, __uint_as_float(v[4 * tq]), __uint_as_float(v[4 * tq + 1]),
-                        __uint_as_float(v[4 * tq + 2]), __uint_as_float(v[4 * tq + 3]));
-      }
-      cluster_sync_all();
-      {
-        const int e = (warp - 2) * 32 + lane;       // 0..127
-        const int rl = e % RS, tg = e / RS;         // row of this CTA's slice, token group
-        const int qpt = RS / 8;                     // token quads per thread: 16 / (128 / RS)
-        const int n_out = n0 + split * RS + rl;     // this CTA's rank in the cluster == its split index
-        const float4 *buf = reinterpret_cast<const float4 *>(sm);
-        __nv_bfloat16 *ob = p.out_bf16 + grp * p.out_group_stride;
-        if (n_out < p.N) {
-          for (int tq = tg * qpt; tq < (tg + 1) * qpt; ++tq) {
-            float4 a = buf[(0 * 16 + tq) * RS + rl];
-            for (int src = 1; src < cs; ++src) {
-              const float4 b = buf[(src * 16 + tq) * RS + rl];
-              a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
-            }
-            const int t0 = 4 * tq;
-            if (t0 < p.rows) ob[(long long)t0 * p.N + n_out] = __float2bfloat16_rn(a.x);
-            if (t0 + 1 < p.rows) ob[(long long)(t0 + 1) * p.N + n_out] = __float2bfloat16_rn(a.y);
-            if (t0 + 2 < p.rows) ob[(long long)(t0 + 2) * p.N + n_out] = __float2bfloat16_rn(a.z);
-            if (t0 + 3 < p.rows) ob[(long long)(t0 + 3) * p.N + n_out] = __float2bfloat16_rn(a.w);
-          }
+      for (int t = 0; t < 32; ++t) {
+        if (tb + t < p.rows) {
+          const float g = q < 2 ? __bfloat162float(__float2bfloat16_rn(__uint_as_float(v[t]))) : __bfloat162float(xg[t * 64 + rr]);
+          const float u = q < 2 ? __bfloat162float(xu[t * 64 + rr]) : __bfloat162float(__float2bfloat16_rn(__uint_as_float(v[32 + t])));
+          const float sg = __bfloat162float(__float2bfloat16_rn(g / (1.f + expf(-g))));
+          p.out_bf16[(long long)(tb + t) * inter + col] = __float2bfloat16_rn(sg * u);
         }
       }
-    } else
-    if (p.silu) {
-      // act(gate) * up (modeling_llama.py:185-186) in the epilogue: lanes 0-63 (warps q = 0, 1) hold gate rows, lanes
-      // 64-127 (q = 2, 3) the up rows of the same 64 output columns.  Each warp pair splits the 64 tokens: the gate warp
-      // finishes tokens 0-31 (it receives the up values through shared memory), the up warp tokens 32-63 (it receives the
-      // gate values), so all four warps share the exponentials.  Rounding points as in eager bf16 (and k_silu_mul):
-      // GEMM out -> bf16, silu -> bf16, product -> bf16.
-      __nv_bfloat16 *xu = reinterpret_cast<__nv_bfloat16 *>(sm + SMEM_BAR + 256);  // up   [32 tokens 0-31 ][64 rows]
-      __nv_bfloat16 *xg = xu + 32 * 64;                                             // gate [32 tokens 32-63][64 rows]
-      const int rr = (q & 1) * 32 + lane;
-      if (q >= 2) {
-#pragma unroll
-        for (int t = 0; t < 32; ++t) xu[t * 64 + rr] = __float2bfloat16_rn(__uint_as_float(v[t]));
-      } else {
-#pragma unroll
-        for (int t = 0; t < 32; ++t) xg[t * 64 + rr] = __float2bfloat16_rn(__uint_as_float(v[32 + t]));
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      const int col = tile * 64 + rr;
-      const int inter = p.N >> 1;
-      if (col < inter) {
-        const int tb = q < 2 ? 0 : 32;
-#pragma unroll
-        for (int t = 0; t < 32; ++t) {
-          if (tb + t < p.rows) {
-            const float g = q < 2 ? __bfloat162float(__float2bfloat16_rn(__uint_as_float(v[t]))) : __bfloat162float(xg[t * 64 + rr]);
-            const float u = q < 2 ? __bfloat162float(xu[t * 64 + rr]) : __bfloat162float(__float2bfloat16_rn(__uint_as_float(v[32 + t])));
-            const float sg = __bfloat162float(__float2bfloat16_rn(g / (1.f + expf(-g))));
-            p.out_bf16[(long long)(tb + t) * inter + col] = __float2bfloat16_rn(sg * u);
-          }
-        }
-      }
-    } else
-    if (n < p.N) {
-      if (p.n_split == 1) {
-#pragma unroll
-        for (int t = 0; t < TOK; ++t)
-          if (t < p.rows) p.out_bf16[grp * p.out_group_stride + (long long)t * p.N + n] = __float2bfloat16_rn(__uint_as_float(v[t]));
-      } else {
-        float *o = p.out_f32 + (long long)split * TOK * p.N;
-#pragma unroll
-        for (int t = 0; t < TOK; ++t)
-          if (t < p.rows) o[(long long)t * p.N + n] = __uint_as_float(v[t]);
-      }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS));
+  } else
+  if (n < p.N) {
+    if (p.n_split == 1) {
+#pragma unroll
+      for (int t = 0; t < TOK; ++t)
+        if (t < p.rows) p.out_bf16[grp * p.out_group_stride + (long long)t * p.N + n] = __float2bfloat16_rn(__uint_as_float(v[t]));
+    } else {
+      float *o = p.out_f32 + (long long)split * TOK * p.N;
+#pragma unroll
+      for (int t = 0; t < TOK; ++t)
+        if (t < p.rows) o[(long long)t * p.N + n] = __uint_as_float(v[t]);
+    }
   }
 }
 
 
 // ------------------------------------------------------------------------------------------------ stream-K
 // Work = n_tiles x n_chunks (tile, k-chunk) units, cut into gridDim.x equal contiguous ranges: every SM streams
-// the same number of bytes whatever N is (qkv: 96 tiles, o/down: 32 tiles on 148 SMs).  A tile whose chunks span
+// the same number of bytes whatever N is (qkv: 96 tiles, o/down: 32 tiles on 132 SMs).  A tile whose chunks span
 // several CTAs is finished by the CTA that holds its FIRST chunk (it reaches that tile last in its own range, so the
 // other contributors - which meet the tile first in theirs - are normally done already): contributors store their
 // fp32 partial to a workspace slot and bump the tile's flag, the owner adds the slots in slot order (deterministic)
@@ -345,39 +356,26 @@ __device__ __forceinline__ int sk_cta_of(long long x, long long U, int G) {
 constexpr int SK_STAGES = 8;
 constexpr int SK_SMEM_BAR = SK_STAGES * STAGE_BYTES;
 constexpr int SK_SMEM_TOTAL = SK_SMEM_BAR + 256 + 1024;
-constexpr int SK_TMEM_COLS = 128;  // two 64-column accumulators
 
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_gemm_sk(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, SkParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t bar_full = base + SK_SMEM_BAR, bar_empty = bar_full + 8 * SK_STAGES, bar_acc_full = bar_empty + 8 * SK_STAGES,
-                 bar_acc_empty = bar_acc_full + 16;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(sm + SK_SMEM_BAR + 16 * SK_STAGES + 48);
+  const uint32_t bar_full = base + SK_SMEM_BAR, bar_empty = bar_full + 8 * SK_STAGES;
   const int G = gridDim.x, b = blockIdx.x;
   const long long u0 = sk_begin(b, p.units, G), u1 = sk_begin(b + 1, p.units, G);
 
   if (tid == 0) {
-    for (int s = 0; s < SK_STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-    mbar_init(bar_acc_full, 1); mbar_init(bar_acc_full + 8, 1);
-    mbar_init(bar_acc_empty, 128); mbar_init(bar_acc_empty + 8, 128);
+    for (int s = 0; s < SK_STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncwarp();  // warp 0 reconverges before the block barrier below
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(SK_TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   pdl_launch_dependents();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       int i = 0;
       for (long long u = u0; u < u1; ++u, ++i) {
@@ -390,108 +388,83 @@ k_gemm_sk(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
         tma_load_2d(xd, &map_x, bar_full + 8 * s, ch * BK, 0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int i = 0, seg = 0;
-      long long u = u0;
-      while (u < u1) {
-        const int tile = (int)(u / p.n_chunks);
-        long long ue = (long long)(tile + 1) * p.n_chunks;
-        if (ue > u1) ue = u1;
-        const int buf = seg & 1;
-        mbar_wait(bar_acc_empty + 8 * buf, ((seg >> 1) & 1) ^ 1);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d = tmem + buf * 64;
-        bool first = true;
-        for (; u < ue; ++u, ++i) {
-          const int s = i % SK_STAGES, ph = (i / SK_STAGES) & 1;
-          mbar_wait(bar_full + 8 * s, ph);
-          tc_fence_after();
-          const uint32_t wa = base + s * STAGE_BYTES, xa = wa + W_BYTES;
+    return;
+  }
+
+  // consumers: one tile segment after the other; the epilogue works on the register fragments directly
+  const int wg = warp >> 2;
+  int i = 0;
+  long long u = u0;
+  float acc[32];
+  while (u < u1) {
+    const int tile = (int)(u / p.n_chunks);
+    const long long ts = (long long)tile * p.n_chunks;
+    long long ue = ts + p.n_chunks;
+    if (ue > u1) ue = u1;
+    const bool head = (u == ts), whole = head && (ue == ts + p.n_chunks);
 #pragma unroll
-          for (int j = 0; j < BK / 16; ++j) {
-            umma_bf16(d, kmajor_desc(wa + j * 32), kmajor_desc(xa + j * 32), IDESC, !(first && j == 0));
-          }
-          first = false;
-          umma_commit(bar_empty + 8 * s);
-        }
-        umma_commit(bar_acc_full + 8 * buf);
-        ++seg;
-      }
+    for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+    for (; u < ue; ++u, ++i) {
+      const int s = i % SK_STAGES, ph = (i / SK_STAGES) & 1;
+      mbar_wait(bar_full + 8 * s, ph);
+      const uint32_t wa = base + s * STAGE_BYTES, xa = wa + W_BYTES;
+      mma_stage(acc, wa + wg * 64 * 128, xa);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * s);
     }
-  } else {
-    // epilogue warps: thread = one weight row of the tile (TMEM lane), 64 token values
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    int seg = 0;
-    long long u = u0;
-    uint32_t v[64];
-    while (u < u1) {
-      const int tile = (int)(u / p.n_chunks);
-      const long long ts = (long long)tile * p.n_chunks;
-      long long ue = ts + p.n_chunks;
-      if (ue > u1) ue = u1;
-      const int buf = seg & 1;
-      mbar_wait(bar_acc_full + 8 * buf, (seg >> 1) & 1);
-      tc_fence_after();
-      const uint32_t a = tmem + buf * 64 + ((uint32_t)(q * 32) << 16);
-      tmem_ld32(a, v);
-      tmem_ld32(a + 32, v + 32);
-      tmem_ld_wait();
-      tc_fence_before();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_acc_empty + 8 * buf) : "memory");
-      const bool head = (u == ts), whole = head && (ue == ts + p.n_chunks);
-      const int n = tile * BMW + r;
-      if (!head) {
-        // contributor: slot = how many CTA ranges after the owner's this one is
-        const int owner = sk_cta_of(ts, p.units, G);
-        const int slot = b - owner - 1;
-        float4 *dst = reinterpret_cast<float4 *>(p.ws + (((long long)tile * p.max_contrib + slot) * BMW + r) * TOK);
+    if (!head) {
+      // contributor: slot = how many CTA ranges after the owner's this one is
+      const int owner = sk_cta_of(ts, p.units, G);
+      const int slot = b - owner - 1;
+      float *ws = p.ws + ((long long)tile * p.max_contrib + slot) * BMW * TOK;
 #pragma unroll
-        for (int t = 0; t < 16; ++t)
-          dst[t] = make_float4(__uint_as_float(v[4 * t]), __uint_as_float(v[4 * t + 1]), __uint_as_float(v[4 * t + 2]),
-                               __uint_as_float(v[4 * t + 3]));
+      for (int h = 0; h < 2; ++h) {
+        const int r = wg * 64 + frag_row(warp, lane, h);
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          *reinterpret_cast<float2 *>(ws + r * TOK + frag_tok(lane, k)) = make_float2(acc[4 * k + 2 * h], acc[4 * k + 2 * h + 1]);
+      }
+      __threadfence();
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (tid == 0) atomicAdd(&p.flags[tile], 1);
+    } else {
+      if (!whole) {
+        // owner: wait for the other contributors of this tile, then add their slots in order
+        const int last = sk_cta_of(ts + p.n_chunks - 1, p.units, G);
+        const int contributors = last - b;
+        if (tid == 0) {
+          while (atomicAdd(&p.flags[tile], 0) < contributors) __nanosleep(64);
+          p.flags[tile] = 0;  // self-reset for the next launch
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
         __threadfence();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (r == 0) atomicAdd(&p.flags[tile], 1);
-      } else {
-        if (!whole) {
-          // owner: wait for the other contributors of this tile, then add their slots in order
-          const int last = sk_cta_of(ts + p.n_chunks - 1, p.units, G);
-          const int contributors = last - b;
-          if (r == 0) {
-            while (atomicAdd(&p.flags[tile], 0) < contributors) __nanosleep(64);
-            p.flags[tile] = 0;  // self-reset for the next launch
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          __threadfence();
-          for (int c = 0; c < contributors; ++c) {
-            const float4 *src = reinterpret_cast<const float4 *>(p.ws + (((long long)tile * p.max_contrib + c) * BMW + r) * TOK);
+        for (int c = 0; c < contributors; ++c) {
+          const float *ws = p.ws + ((long long)tile * p.max_contrib + c) * BMW * TOK;
 #pragma unroll
-            for (int t = 0; t < 16; ++t) {
-              const float4 x = __ldcg(src + t);
-              v[4 * t] = __float_as_uint(__uint_as_float(v[4 * t]) + x.x);
-              v[4 * t + 1] = __float_as_uint(__uint_as_float(v[4 * t + 1]) + x.y);
-              v[4 * t + 2] = __float_as_uint(__uint_as_float(v[4 * t + 2]) + x.z);
-              v[4 * t + 3] = __float_as_uint(__uint_as_float(v[4 * t + 3]) + x.w);
+          for (int h = 0; h < 2; ++h) {
+            const int r = wg * 64 + frag_row(warp, lane, h);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              const float2 x = __ldcg(reinterpret_cast<const float2 *>(ws + r * TOK + frag_tok(lane, k)));
+              acc[4 * k + 2 * h] += x.x;
+              acc[4 * k + 2 * h + 1] += x.y;
             }
           }
         }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int n = tile * BMW + wg * 64 + frag_row(warp, lane, h);
         if (n < p.N) {
 #pragma unroll
-          for (int t = 0; t < TOK; ++t)
-            if (t < p.rows) p.out[(long long)t * p.N + n] = __float2bfloat16_rn(__uint_as_float(v[t]));
+          for (int k = 0; k < 8; ++k) {
+            const int t = frag_tok(lane, k);
+            if (t < p.rows) p.out[(long long)t * p.N + n] = __float2bfloat16_rn(acc[4 * k + 2 * h]);
+            if (t + 1 < p.rows) p.out[(long long)(t + 1) * p.N + n] = __float2bfloat16_rn(acc[4 * k + 2 * h + 1]);
+          }
         }
       }
-      u = ue;
-      ++seg;
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(SK_TMEM_COLS));
   }
 }
 
@@ -593,7 +566,7 @@ extern "C" int pia_gemm_plan_create(const void *d_w, int N, int K, const void *d
                    : encode_2d(&g->map_w, d_w, (uint64_t)K, (uint64_t)N, BK, BMW, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc == PIA_OK) rc = encode_2d(&g->map_x, d_x, (uint64_t)K, (uint64_t)x_rows, BK, TOK, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc == PIA_OK) {
-    int n_sm = 148, dev = 0;
+    int n_sm = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     const int ctas = ((N + BMW - 1) / BMW) * g->p.n_split;
@@ -606,7 +579,7 @@ extern "C" int pia_gemm_plan_create(const void *d_w, int N, int K, const void *d
   if (rc == PIA_OK && want_stream_k) {
     // stream-K over the HBM-tiled weight: grid = min(#SMs, units), fix-up workspace owned by the plan
     if (!w_tiled) { delete g; set_error("stream-K needs the tiled weight layout"); return PIA_ERR_INVALID; }
-    int n_sm = 148, dev = 0;
+    int n_sm = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     SkParams &k = g->sk;
@@ -668,7 +641,7 @@ extern "C" int pia_gemm_plan_create_grouped(const void *d_w, int groups, int N, 
   int rc = encode_2d(&g->map_w, d_w, (uint64_t)K, (uint64_t)groups * N, BK, BMW, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc == PIA_OK) rc = encode_2d(&g->map_x, d_x, (uint64_t)groups * K, (uint64_t)x_rows, BK, TOK, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc == PIA_OK) {
-    int n_sm = 148, dev = 0;
+    int n_sm = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     g->nstage = (N / BMW) * groups <= n_sm ? 8 : 4;

@@ -1,4 +1,4 @@
-// Tree-masked attention for the LOOKAHEAD verify forward (sm_100a: TMA + tcgen05 + TMEM).
+// Tree-masked attention for the LOOKAHEAD verify forward (sm_90a: TMA + wgmma).
 //
 // Takes over the eager attention of the reference's patched models
 //   models/llama/modeling_llama.py:243-308 (QK^T/sqrt(d) + mask, fp32 softmax, PV) with the lookahead mask of
@@ -6,21 +6,19 @@
 // The mask is never materialised: prefix keys [pad_len, P) are visible to every row, the n draft keys follow the
 // row's ancestor bit set (uint64 words, produced by the trie kernel) held in registers.
 //
-// One CTA = (KV split, head group).  A head group is one KV head's worth of rows packed into a single
-// UMMA M=128 tile: 2 query heads x 64 draft rows under GQA, 1 head otherwise (rows 64..127 idle for MHA/64).
-// Warp roles (320 threads):  warp 0 = TMA producer (K/V tiles of 128 keys, 2-stage ring),
-//                            warp 1 = TMEM owner + single-thread tcgen05.mma issuer,
-//                            warps 2-9 = softmax / accumulate, two threads per row (TMEM lane == row; each
-//                            takes 64 S columns and 64 O columns, row max / sum exchanged through smem).
-// Per 128-key tile:  S = Q K^T (8 x UMMA 128x128x16 SS, fp32 in TMEM, double buffered)
-//                    -> hidden keys to -inf (one 32-bit visibility word per 32 keys), online softmax in fp32
-//                    -> P (bf16 pairs) back to TMEM (tcgen05.st, double buffered) = the A operand of
-//                    -> O_tile = P V (8 x UMMA TS form, V consumed MN-major straight from the TMA tile)
-//                    -> acc = acc * alpha + O_tile in registers, one tile late, so that PV(i) and QK^T(i+1) run on
-//                       the tensor core while the softmax warps are busy with tile i+1.
+// One CTA = (KV split, head group).  A head group is one KV head's worth of rows packed into a single 128-row
+// tile: 2 query heads x 64 draft rows under GQA, 1 head otherwise (rows 64..127 idle for MHA/64).
+// Warp roles (288 threads):  warps 0-7 = two consumer warpgroups, each owning 64 rows (wgmma M = 64): they stage Q
+//                            (and, fused, the draft tile), issue the MMAs and run the softmax in registers,
+//                            warp 8 = TMA producer (K/V tiles of 128 keys, 2-stage ring, V on its own barriers).
+// Per 128-key tile and warpgroup:  S = Q K^T (8 x wgmma m64n128k16, both operands from shared memory, fp32 in
+//                    registers) -> hidden keys to -inf (one 32-bit visibility word per 32 keys), online softmax in
+//                    fp32 -> P (bf16 pairs) stays in registers: the S accumulator layout is the A-fragment layout of
+//                    -> O += P V (8 x wgmma m64n128k16, A from registers, V consumed MN-major straight from the
+//                    TMA tile).  The producer keeps the next tile's K/V in flight while a tile is computed.
 // The KV range is split across the CTAs of a thread-block cluster (one wave of clusters, split count decided on the
 // device from the live length): a single-split CTA normalises and writes bf16 directly; otherwise every thread
-// pushes its partial row (acc, m, l) into the shared memory of the CTA that owns the row (DSMEM) and each CTA
+// pushes its partial rows (acc, m, l) into the shared memory of the CTA that owns the row (DSMEM) and each CTA
 // combines its row slice locally - no workspace in HBM, no separate combine launch.
 // HBM-bound by design (arithmetic intensity = rows per KV byte: 64 FLOP/B for MHA, 256 for GQA-4;
 // DESIGN.md gives the roofline).
@@ -36,25 +34,22 @@
 namespace pia {
 namespace attn {
 
-constexpr int BM = 128;      // rows per CTA (UMMA M)
-constexpr int BN = 128;      // keys per tile (UMMA N of QK^T, K extent of PV)
+constexpr int BN = 128;      // keys per tile (wgmma N of QK^T, K extent of PV)
 constexpr int HD = 128;      // head dim
 constexpr int NSTAGE = 2;
-constexpr int NTHREADS = 320;   // warp 0 TMA, warp 1 MMA, warps 2-9 softmax (two warps per TMEM lane quadrant)
+constexpr int NTHREADS = 288;   // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int PRODUCER_WARP = 8;
 constexpr int SUB = 128 * 128;             // bytes of one [128 rows x 64 bf16] swizzle-128B sub-tile
 constexpr int TILE_BYTES = 2 * SUB;        // one 128 x 128 bf16 operand tile
-constexpr int SMEM_Q = 0, SMEM_K = TILE_BYTES, SMEM_V = SMEM_K + NSTAGE * TILE_BYTES;  // P lives in TMEM
+constexpr int SMEM_Q = 0, SMEM_K = TILE_BYTES, SMEM_V = SMEM_K + NSTAGE * TILE_BYTES;
 constexpr int SMEM_BAR = SMEM_V + NSTAGE * TILE_BYTES;
-constexpr int MRG_ACC = 0;                        // [n_split * RS][128] fp32 partial rows pushed by the cluster (over dead Q/P/KV tiles)
+constexpr int MRG_ACC = 0;                        // [n_split * RS][128] fp32 partial rows pushed by the cluster (over dead Q/KV tiles)
 constexpr int MRG_ML = 112 * 1024;                // [n_split * RS] (m, l) pairs
-constexpr int SMEM_XCH = SMEM_BAR + 256;           // row max / row sum exchange between the two column halves
 // merge buffers that never alias a live tile (used when the CTA's rows fit: <= 64 rows): peers may push their
 // partial rows as soon as they are done, without first waiting for this CTA to leave its tile loop
-constexpr int MRG_DED_ACC = SMEM_XCH + 3 * 1024, MRG_DED_ACC_BYTES = (64 + 8) * 128 * 4,  // ns * ceil(64 / ns) <= 64 + MAX_SPLIT - 1 rows
+constexpr int MRG_DED_ACC = SMEM_BAR + 256, MRG_DED_ACC_BYTES = (64 + 8) * 128 * 4,  // ns * ceil(64 / ns) <= 64 + MAX_SPLIT - 1 rows
                MRG_DED_ML = MRG_DED_ACC + MRG_DED_ACC_BYTES;
 constexpr int SMEM_TOTAL = MRG_DED_ML + 1024 + 1024;  // + alignment slack
-constexpr int TMEM_COLS = 512;
-constexpr int TM_S0 = 0, TM_S1 = 128, TM_O = 256, TM_P0 = 384, TM_P1 = 448;  // fp32 S x2, fp32 O, bf16x2-packed P x2
 constexpr int MAX_SPLIT = 8;            // KV splits per head group (merge keeps all partial rows in flight)
 
 // ------------------------------------------------------------------------------------------------ PTX
@@ -86,51 +81,36 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accum) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// registers a wgmma reads or writes asynchronously: pins every later access after the wait above
+__device__ __forceinline__ void fence_regs(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+__device__ __forceinline__ void fence_regs(uint32_t (&a)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
+// D[64 x 128] += A[64 x 16] B[16 x 128]: A = Q (K-major, shared memory), B = K tile (K-major, shared memory)
+__device__ __forceinline__ void wgmma_qk(float (&d)[64], uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accum)
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b)
       : "memory");
 }
-// A operand from TMEM (P, bf16 pairs packed in 32-bit columns, lane == row), B from shared memory
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accum) {
+// D[64 x 128] += P[64 x 16] V[16 x 128]: A = P (bf16 pairs in registers), B = V tile (MN-major, shared memory)
+__device__ __forceinline__ void wgmma_pv(float (&d)[64], const uint32_t *a, uint64_t desc_b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t addr, const uint32_t *v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-        "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-        "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t addr, uint32_t *v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(addr)
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, 1, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b)
       : "memory");
 }
 __device__ __forceinline__ float ex2(float x) {
@@ -148,28 +128,19 @@ __device__ __forceinline__ uint32_t map_to_cta(uint32_t local_smem_addr, uint32_
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(cta_rank));
   return r;
 }
-__device__ __forceinline__ void st_cluster_f4(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
 __device__ __forceinline__ void st_cluster_f2(uint32_t addr, float a, float b) {
   asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// UMMA shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout), SWIZZLE_128B, version 1
+// wgmma shared-memory matrix descriptor (sm_90 GMMA descriptor), SWIZZLE_128B
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;  // LayoutType::SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): bf16 x bf16 -> fp32, M=128, N=128
-__device__ __forceinline__ constexpr uint32_t make_idesc(int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(BN >> 3) << 17) |
-         ((uint32_t)(BM >> 4) << 24);
 }
 
 union Pack8 { uint4 u; __nv_bfloat16 h[8]; };
@@ -222,23 +193,20 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   const uint32_t bar0 = base + SMEM_BAR;
-  const uint32_t bar_kv_full = bar0, bar_kv_empty = bar0 + 8 * NSTAGE, bar_s_full = bar0 + 16 * NSTAGE,
-                 bar_p_full = bar_s_full + 16, bar_o_full = bar_p_full + 16, bar_q_full = bar_o_full + 8,
-                 bar_o_free = bar_q_full + 8, bar_draft = bar_o_free + 8,
-                 bar_v_full = bar0 + 128;  // V tiles complete on their own barriers: QK^T starts as soon as K has landed
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(sm + SMEM_BAR + 16 * NSTAGE + 64);
+  // V tiles complete on their own barriers: QK^T starts as soon as K has landed
+  const uint32_t bar_kv_full = bar0, bar_kv_empty = bar0 + 8 * NSTAGE, bar_v_full = bar0 + 16 * NSTAGE;
 
   pdl_launch_dependents();
-  if (tid == 0) {  // the two TMA descriptors are fetched while the barriers / TMEM are set up
+  if (tid == 0) {  // the two TMA descriptors are fetched while the barriers are set up
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<unsigned long long>(&map_k)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<unsigned long long>(&map_v)) : "memory");
   }
   // Programmatic dependent launch: this CTA may be running while its predecessor (RoPE + KV append of the same layer)
-  // still is.  What is read BEFORE griddepcontrol.wait is safe to read early: d_n / d_prefix_len / d_pad_len / the mask
-  // rows were written before the first kernel of the layer chain (trie get and the previous step's accept are launched
-  // without the PDL attribute, prefill meta is a stream-ordered copy), and cache rows below P were written by earlier
-  // steps.  Only Q, the rows [P, P + n) of this layer's K/V planes and the output buffer depend on the predecessor: the
-  // TMA producer waits before its first tile that reaches row P, the softmax warps wait before they read Q.
+  // still is.  What is read BEFORE griddepcontrol.wait is safe to read early: d_n / d_prefix_len / d_pad_len were
+  // written before the first kernel of the layer chain (trie get and the previous step's accept are launched without
+  // the PDL attribute, prefill meta is a stream-ordered copy), and cache rows below P were written by earlier steps.
+  // Only Q, the rows [P, P + n) of this layer's K/V planes and the output buffer depend on the predecessor: the TMA
+  // producer waits before its first tile that reaches row P, the consumer warps wait before they read Q.
   const int split = blockIdx.x, group = blockIdx.y;
   const int slot = blockIdx.z;
   const int n = p.sl.d_n[slot], P = p.sl.d_prefix_len[slot];
@@ -249,13 +217,14 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
   const int hq0 = group * p.heads_per_cta;
   const int hkv = hq0 / (p.n_q_heads / p.n_kv_heads);
   // tiles: plain mode = the keys [0, L) of the cache; fused mode = the prefix tiles [0, P) of the cache + ONE draft tile
-  // (the n draft keys, rotated and staged in shared memory by the softmax warps of the CTA that owns the last tile)
+  // (the n draft keys, rotated and staged in shared memory by the consumer warps of the CTA that owns the last tile)
   const bool fused = p.fused != 0;
   const int Tp = (P + BN - 1) / BN;
   const int tiles_total = fused ? Tp + 1 : (L + BN - 1) / BN;
   // Work split decided on the device from the live length: tiles_per_cta tiles per CTA (more only when the
   // plan's split limit is reached); a single split writes the final output directly (no partials, no merge).
   const int rows_used = p.heads_per_cta * p.np;          // 64 (MHA, 64 nodes) or 128
+  const int n_wg = rows_used / 64;                       // consumer warpgroups with live rows
   const bool ded = (rows_used + MAX_SPLIT) * HD * 4 <= MRG_DED_ACC_BYTES;
   int ns = (tiles_total + p.tiles_per_cta - 1) / p.tiles_per_cta;
   if (ns > p.n_split) ns = p.n_split;
@@ -280,37 +249,21 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
   auto barrier_a = [&]() { if (ded) cluster_wait(); else cluster_sync_all(); };
   const int mrg_acc = ded ? MRG_DED_ACC : MRG_ACC, mrg_ml = ded ? MRG_DED_ML : MRG_ML;
   const int mrg_stride = ded ? 64 + MAX_SPLIT : 128 + MAX_SPLIT;  // slots per chunk column
-  const bool is_sm_warp = warp >= 2;
-  const int half = is_sm_warp ? (warp - 2) >> 2 : 0;     // which 64 columns of S / O this softmax warp owns
-  const int row = ((warp & 3) << 5) | lane;              // TMEM lane == row (a warp may only touch its quadrant)
-  const bool warp_active = is_sm_warp && (((warp & 3) << 5) < rows_used);
-  const int hs = row / p.np, node = row % p.np;
-  const bool row_live = warp_active && node < n;
   if (tid == 0) DBG(0);
 
   // ---- setup
   if (tid == 0) {
-    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar_kv_full + 8 * s, 1); mbar_init(bar_kv_empty + 8 * s, 1); mbar_init(bar_v_full + 8 * s, 1); }
-    mbar_init(bar_s_full, 1); mbar_init(bar_s_full + 8, 1);
-    mbar_init(bar_p_full, 2 * rows_used); mbar_init(bar_p_full + 8, 2 * rows_used);
-    mbar_init(bar_o_free, 2 * rows_used);
-    mbar_init(bar_o_full, 1);
-    mbar_init(bar_q_full, 2 * rows_used);
-    mbar_init(bar_draft, NTHREADS - 64);  // all eight softmax warps stage the draft tile
+    for (int s = 0; s < NSTAGE; ++s) {
+      mbar_init(bar_kv_full + 8 * s, 1); mbar_init(bar_v_full + 8 * s, 1);
+      mbar_init(bar_kv_empty + 8 * s, 4 * n_wg);  // one arrive per consumer warp with live rows
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncwarp();  // warp 0 reconverges before the (warp-aligned) block barrier below (synccheck: divergent lane 0)
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
+  __syncwarp();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   if (tid == 0) DBG(1);
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ================================================================ TMA producer
     if (lane == 0 && ntile > 0) {
       const int plane = p.plane0 + slot * p.slot_planes + p.layer * p.n_kv_heads + hkv;
@@ -321,7 +274,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
       bool waited = false;
       for (int i = 0; i < ntile; ++i) {
         const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
-        if (has_draft && i == 0) {  // staged by the softmax warps (bar_draft); this arrive only keeps the phases aligned
+        if (has_draft && i == 0) {  // staged by the consumer warps; this arrive only keeps the phases aligned
           mbar_arrive(bar_kv_full);
           mbar_arrive(bar_v_full);
           continue;
@@ -343,325 +296,304 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
     }
     __syncwarp();
     if (ns > 1) { barrier_a(); cluster_sync_all(); }
-  } else if (warp == 1) {
-    // ================================================================ MMA issuer (one thread)
-    if (lane == 0 && ntile > 0) {
-      constexpr uint32_t IDESC_QK = make_idesc(0), IDESC_PV = make_idesc(1);
-      mbar_wait(bar_q_full, 0);
-      auto issue_qk = [&](int i) {
+  } else {
+    pdl_wait();  // Q (or, fused, the projection output) below is the predecessor's output
+    // ================================================================ staging: thread = (tile row srow, 64-wide half)
+    {
+      const int srow = tid & 127, half = tid >> 7;
+      const int hs = srow / p.np, node = srow % p.np;
+      if (srow < rows_used) {
+        if (!fused) {
+          uint4 qv[8];  // Q row -> shared memory (K-major SWIZZLE_128B); each half loads one 64-wide d sub-tile
+          const bool have = hs < p.heads_per_cta && node < n;
+          const uint4 *src = reinterpret_cast<const uint4 *>(p.q + ((row0 + node) * p.n_q_heads + hq0 + hs) * HD) + half * 8;
+#pragma unroll
+          for (int ch = 0; ch < 8; ++ch) qv[ch] = have ? src[ch] : make_uint4(0, 0, 0, 0);
+#pragma unroll
+          for (int ch = 0; ch < 8; ++ch)
+            *reinterpret_cast<uint4 *>(sm + SMEM_Q + half * SUB + srow * 128 + ((ch ^ (srow & 7)) << 4)) = qv[ch];
+        } else {
+          unsigned long long mr0 = 0ull, mr1 = 0ull;
+          if (node < n) {
+            mr0 = p.mask[(row0 + node) * p.mask_words];
+            if (p.mask_words > 1) mr1 = p.mask[(row0 + node) * p.mask_words + 1];
+          }
+          // RoPE at the node's position = rowsum(mask) - 1 (modeling_llama.py:587): visible prefix + tree depth
+          int pos = (P > pad_len ? P - pad_len : 0) + __popcll(mr0) + __popcll(mr1) - 1;
+          pos = pos < 0 ? 0 : (pos >= p.max_pos ? p.max_pos - 1 : pos);
+          const uint4 *cs = reinterpret_cast<const uint4 *>(p.cos_t + (long long)pos * (HD / 2));
+          const uint4 *sn = reinterpret_cast<const uint4 *>(p.sin_t + (long long)pos * (HD / 2));
+          const long long row_elems = (long long)(p.n_q_heads + 2 * p.n_kv_heads) * HD;
+          const __nv_bfloat16 *xr = p.qkv + (row0 + node) * row_elems;
+          const bool have = hs < p.heads_per_cta && node < n;
+          // All global loads of a batch are issued (read-only path: the compiler may not move plain loads across the
+          // shared memory stores in between, and eight dependent load rounds would serialise the prologue) before the
+          // first value is used; four 16-byte chunks per batch bound the registers.
+          {  // Q: rotate this thread's 64-wide half (the other half of the head is the rotation partner)
+            const uint4 *qa = reinterpret_cast<const uint4 *>(xr + (long long)(hq0 + hs) * HD) + half * 8;
+            const uint4 *qb = reinterpret_cast<const uint4 *>(xr + (long long)(hq0 + hs) * HD) + (half ^ 1) * 8;
+#pragma unroll
+            for (int b4 = 0; b4 < 2; ++b4) {
+              uint4 ra[4], rb[4], rc[4], rs[4];
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const int ch = b4 * 4 + j;
+                if (have) { ra[j] = __ldg(qa + ch); rb[j] = __ldg(qb + ch); rc[j] = __ldg(cs + ch); rs[j] = __ldg(sn + ch); }
+              }
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const int ch = b4 * 4 + j;
+                const uint4 o = have ? rope8(ra[j], rb[j], rc[j], rs[j], half == 0) : make_uint4(0, 0, 0, 0);
+                *reinterpret_cast<uint4 *>(sm + SMEM_Q + half * SUB + srow * 128 + ((ch ^ (srow & 7)) << 4)) = o;
+              }
+            }
+          }
+          if (has_draft) {
+            // the draft tile (ring slot 0): key row r = draft node r, K rotated at r's position, V as projected; rows
+            // that hold no node are zero.  The threads of the tile's first head (hs == 0: srow == node) own the key
+            // rows; one CTA per KV head also appends the rows to the cache for the steps to come (pretrained_model.py:
+            // the reference's torch.cat of past and new K/V, modeling_llama.py:265-268)
+            const bool key_row = hs == 0 && node < n;
+            const bool writer = (hq0 % (p.n_q_heads / p.n_kv_heads)) == 0;
+            const uint4 *ka = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + half * 8;
+            const uint4 *kb = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + (half ^ 1) * 8;
+            const uint4 *va = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + p.n_kv_heads + hkv) * HD) + half * 8;
+            const long long crow = (long long)slot * p.sl.kv_slot_stride + ((long long)hkv * p.max_seq + P + node) * HD + half * 64;
+            uint4 *kdst = reinterpret_cast<uint4 *>(p.kc_layer + crow), *vdst = reinterpret_cast<uint4 *>(p.vc_layer + crow);
+#pragma unroll
+            for (int b4 = 0; b4 < 2; ++b4) {
+              uint4 ra[4], rb[4], rc[4], rs[4], rv[4];
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const int ch = b4 * 4 + j;
+                if (key_row) {
+                  ra[j] = __ldg(ka + ch); rb[j] = __ldg(kb + ch); rc[j] = __ldg(cs + ch); rs[j] = __ldg(sn + ch);
+                  rv[j] = __ldg(va + ch);
+                }
+              }
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const int ch = b4 * 4 + j;
+                const uint32_t off = half * SUB + srow * 128 + ((ch ^ (srow & 7)) << 4);
+                uint4 ko = make_uint4(0, 0, 0, 0), vo = make_uint4(0, 0, 0, 0);
+                if (key_row) { ko = rope8(ra[j], rb[j], rc[j], rs[j], half == 0); vo = rv[j]; }
+                *reinterpret_cast<uint4 *>(sm + SMEM_K + off) = ko;
+                *reinterpret_cast<uint4 *>(sm + SMEM_V + off) = vo;
+                if (key_row && writer) { kdst[ch] = ko; vdst[ch] = vo; }
+              }
+            }
+          }
+        }
+      } else if (has_draft) {
+        // rows 64..127 of a 64-row tile: the draft tile's key rows there are never live, they are zeroed
+#pragma unroll
+        for (int ch = 0; ch < 8; ++ch) {
+          const uint32_t off = half * SUB + srow * 128 + ((ch ^ (srow & 7)) << 4);
+          *reinterpret_cast<uint4 *>(sm + SMEM_K + off) = make_uint4(0, 0, 0, 0);
+          *reinterpret_cast<uint4 *>(sm + SMEM_V + off) = make_uint4(0, 0, 0, 0);
+        }
+      }
+      fence_async_smem();  // generic-proxy stores -> visible to the wgmma (async proxy) reads
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (tid == 0) DBG(5);
+
+    const int wg = warp >> 2;
+    if (wg < n_wg) {
+      // ================================================================ QK^T, softmax, PV of this warpgroup's 64 rows
+      // accumulator fragments: register 4 * nb + 2 * h + e holds row rw[h] = 64 wg + 16 (warp % 4) + lane / 4 + 8 h,
+      // column 8 nb + 2 (lane % 4) + e (a key of S, a head-dim element of O)
+      int rw[2], hs[2], node[2];
+      bool live[2];
+      unsigned long long mrow[2][2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        rw[h] = wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+        hs[h] = rw[h] / p.np; node[h] = rw[h] % p.np;
+        live[h] = node[h] < n;
+        mrow[h][0] = mrow[h][1] = 0ull;
+        if (live[h]) {
+          mrow[h][0] = p.mask[(row0 + node[h]) * p.mask_words];
+          if (p.mask_words > 1) mrow[h][1] = p.mask[(row0 + node[h]) * p.mask_words + 1];
+        }
+      }
+      const uint32_t qa = base + SMEM_Q + wg * 64 * 128;
+      float o[64];
+#pragma unroll
+      for (int j = 0; j < 64; ++j) o[j] = 0.f;
+      float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // l_run: this thread's 32 columns of the row
+      for (int i = 0; i < ntile; ++i) {
+        const int tl = tile_of(i);
+        const bool is_draft = fused && tl == Tp;
         const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
+        const uint32_t ka = base + SMEM_K + s * TILE_BYTES, va = base + SMEM_V + s * TILE_BYTES;
         mbar_wait(bar_kv_full + 8 * s, ph);
-        if (has_draft && i == 0) mbar_wait(bar_draft, 0);
-        tc_fence_after();
-        const uint32_t qa = base + SMEM_Q, ka = base + SMEM_K + s * TILE_BYTES;
-        const uint32_t d = tmem + ((i & 1) ? TM_S1 : TM_S0);
+        float sv[64];
+#pragma unroll
+        for (int j = 0; j < 64; ++j) sv[j] = 0.f;
+        wgmma_fence();
 #pragma unroll
         for (int j = 0; j < HD / 16; ++j) {  // K-major operands: 32 B per k-block inside the 128 B swizzle row
           const uint32_t off = (j >> 2) * SUB + (j & 3) * 32;
-          umma_bf16(d, make_desc(qa + off, 16, 1024), make_desc(ka + off, 16, 1024), IDESC_QK, j > 0);
+          wgmma_qk(sv, make_desc(qa + off, 16, 1024), make_desc(ka + off, 16, 1024));
         }
-        umma_commit(bar_s_full + 8 * (i & 1));
-      };
-      issue_qk(0);
-      DBG(3);
-      for (int i = 0; i < ntile; ++i) {
-        if (i + 1 < ntile) issue_qk(i + 1);  // S is double buffered: next QK^T overlaps this tile's softmax
-        const int s = i % NSTAGE;
-        mbar_wait(bar_p_full + 8 * (i & 1), (i >> 1) & 1);
-        if (i > 0) mbar_wait(bar_o_free, (i - 1) & 1);  // the softmax warps have folded O(i-1) into their registers
-        mbar_wait(bar_v_full + 8 * s, (i / NSTAGE) & 1);
-        tc_fence_after();
-        const uint32_t va = base + SMEM_V + s * TILE_BYTES;
-        const uint32_t pa = tmem + ((i & 1) ? TM_P1 : TM_P0);
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_regs(sv);
+        if (tid == 0 && i == 0) DBG(6);
+        // 32-bit visibility word of keys [kb, kb+32): prefix keys [pad_len, P) are visible to every row, the n draft
+        // keys follow the row's ancestor bits (bits beyond the live nodes are never set in the trie's mask rows)
+        const bool all_visible = !is_draft && (tl * BN >= pad_len) && (tl * BN + BN <= P);
+        if (!all_visible) {  // tree / padded / ragged tile: hidden keys -> -inf once, then the dense code
 #pragma unroll
-        for (int j = 0; j < BN / 16; ++j) {
-          // A = P from TMEM (16 keys = 8 packed columns per k-block); B = V, MN-major: 16 keys = 2 groups of 8 rows
-          // (SBO 1024 B), d-halves 16 KB apart (LBO)
-          umma_bf16_ts(tmem + TM_O, pa + j * 8, make_desc(va + j * 2048, SUB, 1024), IDESC_PV, j > 0);
-        }
-        umma_commit(bar_o_full);
-        umma_commit(bar_kv_empty + 8 * s);
-      }
-      DBG(4);
-    }
-    __syncwarp();
-    if (ns > 1) { barrier_a(); cluster_sync_all(); }
-  } else if (fused && !warp_active) {
-    // ================================================================ idle softmax warps of a 64-row tile, fused mode:
-    // they zero the draft tile's key rows 64..127 (never live when the tile holds 64 nodes)
-    if (has_draft) {
+          for (int h = 0; h < 2; ++h) {
+            const unsigned long long m0 = mrow[h][0], m1 = mrow[h][1];
+            auto vis32 = [&](int kb) -> uint32_t {
+              if (is_draft) {  // key kb - Tp * BN is draft node j0: visible iff it is an ancestor (or the node itself)
+                const int j0 = kb - Tp * BN;
+                if (j0 < 64) {
+                  unsigned long long x = m0 >> j0;
+                  if (j0 > 32) x |= m1 << (64 - j0);
+                  return (uint32_t)x;
+                }
+                return (uint32_t)(m1 >> (j0 - 64));
+              }
+              uint32_t m = 0;
+              const int lo = kb < pad_len ? pad_len : kb;
+              const int hi = kb + 32 < P ? kb + 32 : P;
+              if (hi > lo) m = (hi - lo >= 32 ? 0xffffffffu : ((1u << (hi - lo)) - 1u)) << (lo - kb);
+              const int j0 = kb - P;
+              if (!fused && j0 + 32 > 0 && j0 < n) {
+                uint32_t d;
+                if (j0 < 0) d = (uint32_t)(m0 << (-j0));
+                else if (j0 < 64) {
+                  unsigned long long x = m0 >> j0;
+                  if (j0 > 32) x |= m1 << (64 - j0);
+                  d = (uint32_t)x;
+                } else d = (uint32_t)(m1 >> (j0 - 64));
+                m |= d;
+              }
+              return m;
+            };
 #pragma unroll
-      for (int ch = 0; ch < 8; ++ch) {
-        const uint32_t off = half * SUB + row * 128 + ((ch ^ (row & 7)) << 4);
-        *reinterpret_cast<uint4 *>(sm + SMEM_K + off) = make_uint4(0, 0, 0, 0);
-        *reinterpret_cast<uint4 *>(sm + SMEM_V + off) = make_uint4(0, 0, 0, 0);
-      }
-      fence_async_smem();
-      mbar_arrive(bar_draft);
-    }
-    if (ns > 1) { barrier_a(); cluster_sync_all(); }
-  } else if (warp_active) {
-    // ================================================================ softmax + accumulate
-    // two threads per row: `half` selects 64 of the 128 S columns (keys) and 64 of the 128 O columns (head dim)
-    pdl_wait();  // Q (or, fused, the projection output) below is the predecessor's output
-    unsigned long long mrow[2] = {0ull, 0ull};
-    if (row_live) {
-      mrow[0] = p.mask[(row0 + node) * p.mask_words];
-      if (p.mask_words > 1) mrow[1] = p.mask[(row0 + node) * p.mask_words + 1];
-    }
-    if (!fused) {
-      uint4 qv[8];  // Q row -> shared memory (UMMA K-major SWIZZLE_128B); each half loads one 64-wide d sub-tile
-      const bool have = hs < p.heads_per_cta && node < n;
-      const uint4 *src = reinterpret_cast<const uint4 *>(p.q + ((row0 + node) * p.n_q_heads + hq0 + hs) * HD) + half * 8;
+            for (int c = 0; c < 4; ++c) {
+              const uint32_t vm = vis32(tl * BN + 32 * c) >> (2 * (lane & 3));
 #pragma unroll
-      for (int ch = 0; ch < 8; ++ch) qv[ch] = have ? src[ch] : make_uint4(0, 0, 0, 0);
-#pragma unroll
-      for (int ch = 0; ch < 8; ++ch)
-        *reinterpret_cast<uint4 *>(sm + SMEM_Q + half * SUB + row * 128 + ((ch ^ (row & 7)) << 4)) = qv[ch];
-      fence_async_smem();
-      mbar_arrive(bar_q_full);
-    } else {
-      // RoPE at the node's position = rowsum(mask) - 1 (modeling_llama.py:587): visible prefix + tree depth
-      int pos = (P > pad_len ? P - pad_len : 0) + __popcll(mrow[0]) + __popcll(mrow[1]) - 1;
-      pos = pos < 0 ? 0 : (pos >= p.max_pos ? p.max_pos - 1 : pos);
-      const uint4 *cs = reinterpret_cast<const uint4 *>(p.cos_t + (long long)pos * (HD / 2));
-      const uint4 *sn = reinterpret_cast<const uint4 *>(p.sin_t + (long long)pos * (HD / 2));
-      const long long row_elems = (long long)(p.n_q_heads + 2 * p.n_kv_heads) * HD;
-      const __nv_bfloat16 *xr = p.qkv + (row0 + node) * row_elems;
-      const bool have = hs < p.heads_per_cta && node < n;
-      // All global loads of a batch are issued (read-only path: the compiler may not move plain loads across the shared
-      // memory stores in between, and eight dependent load rounds of ~0.7 us each would serialise the prologue) before
-      // the first value is used; four 16-byte chunks per batch bound the registers.
-      {  // Q: rotate this thread's 64-wide half (the other half of the head is the rotation partner)
-        const uint4 *qa = reinterpret_cast<const uint4 *>(xr + (long long)(hq0 + hs) * HD) + half * 8;
-        const uint4 *qb = reinterpret_cast<const uint4 *>(xr + (long long)(hq0 + hs) * HD) + (half ^ 1) * 8;
-#pragma unroll
-        for (int b4 = 0; b4 < 2; ++b4) {
-          uint4 ra[4], rb[4], rc[4], rs[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int ch = b4 * 4 + j;
-            if (have) { ra[j] = __ldg(qa + ch); rb[j] = __ldg(qb + ch); rc[j] = __ldg(cs + ch); rs[j] = __ldg(sn + ch); }
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int ch = b4 * 4 + j;
-            const uint4 o = have ? rope8(ra[j], rb[j], rc[j], rs[j], half == 0) : make_uint4(0, 0, 0, 0);
-            *reinterpret_cast<uint4 *>(sm + SMEM_Q + half * SUB + row * 128 + ((ch ^ (row & 7)) << 4)) = o;
-          }
-        }
-        fence_async_smem();
-        mbar_arrive(bar_q_full);
-      }
-      if (has_draft) {
-        // the draft tile (ring slot 0): key row r = draft node r, K rotated at r's position, V as projected; rows that
-        // hold no node are zero.  The threads of the tile's first head (hs == 0: row == node) own the key rows; one CTA
-        // per KV head also appends the rows to the cache for the steps to come (pretrained_model.py: the reference's
-        // torch.cat of past and new K/V, modeling_llama.py:265-268)
-        const bool key_row = hs == 0 && node < n;
-        const bool writer = (hq0 % (p.n_q_heads / p.n_kv_heads)) == 0;
-        const uint4 *ka = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + half * 8;
-        const uint4 *kb = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + (half ^ 1) * 8;
-        const uint4 *va = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + p.n_kv_heads + hkv) * HD) + half * 8;
-        const long long crow = (long long)slot * p.sl.kv_slot_stride + ((long long)hkv * p.max_seq + P + node) * HD + half * 64;
-        uint4 *kdst = reinterpret_cast<uint4 *>(p.kc_layer + crow), *vdst = reinterpret_cast<uint4 *>(p.vc_layer + crow);
-#pragma unroll
-        for (int b4 = 0; b4 < 2; ++b4) {
-          uint4 ra[4], rb[4], rc[4], rs[4], rv[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int ch = b4 * 4 + j;
-            if (key_row) {
-              ra[j] = __ldg(ka + ch); rb[j] = __ldg(kb + ch); rc[j] = __ldg(cs + ch); rs[j] = __ldg(sn + ch);
-              rv[j] = __ldg(va + ch);
+              for (int k = 0; k < 4; ++k) {
+                const int nb = 4 * c + k;
+                if (!((vm >> (8 * k)) & 1u)) sv[4 * nb + 2 * h] = -INFINITY;
+                if (!((vm >> (8 * k + 1)) & 1u)) sv[4 * nb + 2 * h + 1] = -INFINITY;
+              }
             }
           }
+        }
+        // row max: this thread's 32 columns, then the four lanes that share the row
+        float m_new[2], m_use[2], alpha[2];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int ch = b4 * 4 + j;
-            const uint32_t off = half * SUB + row * 128 + ((ch ^ (row & 7)) << 4);
-            uint4 ko = make_uint4(0, 0, 0, 0), vo = make_uint4(0, 0, 0, 0);
-            if (key_row) { ko = rope8(ra[j], rb[j], rc[j], rs[j], half == 0); vo = rv[j]; }
-            *reinterpret_cast<uint4 *>(sm + SMEM_K + off) = ko;
-            *reinterpret_cast<uint4 *>(sm + SMEM_V + off) = vo;
-            if (key_row && writer) { kdst[ch] = ko; vdst[ch] = vo; }
+        for (int h = 0; h < 2; ++h) {
+          float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+          for (int nb = 0; nb < 16; ++nb) {
+            mx0 = fmaxf(mx0, sv[4 * nb + 2 * h]);
+            mx1 = fmaxf(mx1, sv[4 * nb + 2 * h + 1]);
+          }
+          float mx = fmaxf(mx0, mx1);
+          mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 2));
+          m_new[h] = fmaxf(m_run[h], mx * p.scale_log2);
+          m_use[h] = (m_new[h] == -INFINITY) ? 0.f : m_new[h];
+          alpha[h] = (m_run[h] == -INFINITY) ? 0.f : ex2(m_run[h] - m_use[h]);
+        }
+        // p = exp2(s*scale - m) -> bf16 pairs: register pair (2 m, 2 m + 1) of S is A-fragment register m of PV
+        // (k-block m / 4), so P never leaves the registers; the row sum uses the bf16-rounded probabilities, i.e.
+        // exactly what the PV MMA consumes
+        uint32_t pa[32];
+        float ls[2] = {0.f, 0.f};
+#pragma unroll
+        for (int m = 0; m < 32; ++m) {  // ex2(-inf) = 0 for the hidden keys (m_use is finite)
+          const int h = m & 1;
+          const float p0 = ex2(sv[2 * m] * p.scale_log2 - m_use[h]);
+          const float p1 = ex2(sv[2 * m + 1] * p.scale_log2 - m_use[h]);
+          const __nv_bfloat162 b = __floats2bfloat162_rn(p0, p1);
+          ls[h] += __bfloat162float(b.x) + __bfloat162float(b.y);
+          pa[m] = *reinterpret_cast<const uint32_t *>(&b);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          l_run[h] = l_run[h] * alpha[h] + ls[h];
+          m_run[h] = m_new[h];
+        }
+#pragma unroll
+        for (int nb = 0; nb < 16; ++nb) {
+          o[4 * nb] *= alpha[0]; o[4 * nb + 1] *= alpha[0];
+          o[4 * nb + 2] *= alpha[1]; o[4 * nb + 3] *= alpha[1];
+        }
+        if (tid == 0 && i == 0) DBG(7);
+        mbar_wait(bar_v_full + 8 * s, ph);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < BN / 16; ++j) {
+          // B = V, MN-major: 16 keys = 2 groups of 8 rows (SBO 1024 B), d-halves 16 KB apart (LBO)
+          wgmma_pv(o, pa + 4 * j, make_desc(va + j * 2048, SUB, 1024));
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_regs(o);
+        fence_regs(pa);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_kv_empty + 8 * s);  // this warp is done with the stage's K and V
+      }
+      if (tid == 0) DBG(8);
+      // total row sum = the four lanes of the row (same running max, so the partial sums just add)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        l_run[h] += __shfl_xor_sync(FULL, l_run[h], 1);
+        l_run[h] += __shfl_xor_sync(FULL, l_run[h], 2);
+      }
+      if (tid == 0) DBG(9);
+      if (ns == 1) {
+        // single split: normalise and write the final bf16 rows
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (live[h]) {
+            const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
+            uint32_t *dst = reinterpret_cast<uint32_t *>(p.out + ((row0 + node[h]) * p.n_q_heads + hq0 + hs[h]) * HD);
+#pragma unroll
+            for (int nb = 0; nb < 16; ++nb) {
+              __nv_bfloat162 b = __floats2bfloat162_rn(o[4 * nb + 2 * h] * inv, o[4 * nb + 2 * h + 1] * inv);
+              dst[4 * nb + (lane & 3)] = *reinterpret_cast<uint32_t *>(&b);
+            }
           }
         }
-        fence_async_smem();
-        mbar_arrive(bar_draft);
-      }
-    }
-    if (row == 0 && half == 0) DBG(5);
-    const uint32_t lane_addr = (uint32_t)((warp & 3) * 32) << 16;
-    const int pair_bar = 1 + (warp & 3);  // named barrier shared by the two warps of this lane quadrant
-    float acc[64];
+      } else {
+        // several splits: the ns CTAs of this head group form one thread-block cluster.  After everyone has left its
+        // tile loop (barrier A: the Q/KV tiles of every CTA are dead) each thread pushes its rows' pieces - acc, and
+        // the row's (m, l) - straight into the shared memory of the CTA that owns that row's slice (DSMEM), barrier B,
+        // and every CTA combines its slice locally: no workspace round trip through L2, no serial last-arriver merge.
+        barrier_a();
+        if (tid == 0) DBG(14);
+        const int RS = (rows_used + ns - 1) / ns;       // rows per owner CTA
 #pragma unroll
-    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f, alpha_prev = 0.f;
-    uint32_t sv[64];
-    for (int i = 0; i < ntile; ++i) {
-      const int tl = tile_of(i);
-      const bool is_draft = fused && tl == Tp;
-      const int key0 = tl * BN + half * 64;
-      const uint32_t s_addr = tmem + lane_addr + ((i & 1) ? TM_S1 : TM_S0) + half * 64;
-      mbar_wait(bar_s_full + 8 * (i & 1), (i >> 1) & 1);
-      tc_fence_after();
-      if (row == 0 && half == 0 && i == 0) DBG(6);
-      tmem_ld32(s_addr, sv);
-      tmem_ld32(s_addr + 32, sv + 32);
-      tmem_ld_wait();
-      // 32-bit visibility word of keys [kb, kb+32): prefix keys [pad_len, P) are visible to every row, the n draft
-      // keys follow the row's ancestor bits (bits beyond the live nodes are never set in the trie's mask rows)
-      const bool all_visible = !is_draft && (tl * BN >= pad_len) && (tl * BN + BN <= P);
-      auto vis32 = [&](int kb) -> uint32_t {
-        if (all_visible) return 0xffffffffu;
-        if (is_draft) {  // key kb - Tp * BN is draft node j0: visible iff it is an ancestor (or the node itself)
-          const int j0 = kb - Tp * BN;
-          if (j0 < 64) {
-            unsigned long long x = mrow[0] >> j0;
-            if (j0 > 32) x |= mrow[1] << (64 - j0);
-            return (uint32_t)x;
+        for (int h = 0; h < 2; ++h) {
+          if (live[h]) {
+            const int owner = rw[h] / RS, rl = rw[h] % RS;
+            // partial rows are stored chunk-major ([32 float4 chunks][slot]): head-dim element d = 8 nb + 2 (lane % 4)
+            // lies in chunk d / 4 = 2 nb + (lane % 4) / 2, at float offset 2 (lane % 2)
+            const uint32_t dst = map_to_cta(base + mrg_acc + (uint32_t)((((lane & 3) >> 1) * mrg_stride + split * RS + rl) * 16 + (lane & 1) * 8), owner);
+#pragma unroll
+            for (int nb = 0; nb < 16; ++nb)
+              st_cluster_f2(dst + (uint32_t)(2 * nb * mrg_stride) * 16, o[4 * nb + 2 * h], o[4 * nb + 2 * h + 1]);
+            if ((lane & 3) == 0) st_cluster_f2(map_to_cta(base + mrg_ml + (uint32_t)(split * RS + rl) * 8, owner), m_run[h], l_run[h]);
           }
-          return (uint32_t)(mrow[1] >> (j0 - 64));
         }
-        uint32_t m = 0;
-        const int lo = kb < pad_len ? pad_len : kb;
-        const int hi = kb + 32 < P ? kb + 32 : P;
-        if (hi > lo) m = (hi - lo >= 32 ? 0xffffffffu : ((1u << (hi - lo)) - 1u)) << (lo - kb);
-        const int j0 = kb - P;
-        if (!fused && j0 + 32 > 0 && j0 < n) {
-          uint32_t d;
-          if (j0 < 0) d = (uint32_t)(mrow[0] << (-j0));
-          else if (j0 < 64) {
-            unsigned long long x = mrow[0] >> j0;
-            if (j0 > 32) x |= mrow[1] << (64 - j0);
-            d = (uint32_t)x;
-          } else d = (uint32_t)(mrow[1] >> (j0 - 64));
-          m |= d;
-        }
-        return m;
-      };
-      const uint32_t vm0 = vis32(key0), vm1 = vis32(key0 + 32);
-      if ((vm0 & vm1) != 0xffffffffu) {  // tree / padded / ragged tile: hidden keys -> -inf once, then the dense code
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          if (!((vm0 >> j) & 1u)) sv[j] = 0xff800000u;
-          if (!((vm1 >> j) & 1u)) sv[32 + j] = 0xff800000u;
-        }
+        __syncwarp();  // the live-row branch above diverges; the cluster barrier is warp-aligned
+        if (tid == 0) DBG(15);
+        cluster_sync_all();
       }
-      // four independent chains (a single 64-long fmaxf / FADD chain is ~250 cycles of pure latency per tile)
-      float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-      for (int j = 0; j < 64; j += 4) {
-        mx0 = fmaxf(mx0, __uint_as_float(sv[j])); mx1 = fmaxf(mx1, __uint_as_float(sv[j + 1]));
-        mx2 = fmaxf(mx2, __uint_as_float(sv[j + 2])); mx3 = fmaxf(mx3, __uint_as_float(sv[j + 3]));
-      }
-      const float m_half = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-      // row max across the two halves (double-buffered exchange slot, one named barrier per quadrant pair)
-      float *xm = reinterpret_cast<float *>(sm + SMEM_XCH) + (i & 1) * 256;
-      xm[half * 128 + row] = m_half;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      const float m_tile = fmaxf(m_half, xm[(half ^ 1) * 128 + row]);
-      const float m_new = fmaxf(m_run, m_tile * p.scale_log2);
-      const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-      const float alpha = (m_run == -INFINITY) ? 0.f : ex2(m_run - m_use);
-      // p = exp2(s*scale - m) -> bf16 pairs -> TMEM (A operand of the PV MMA: lane = row, one 32-bit column per key
-      // pair; this half owns columns [32*half, 32*half+32)), row sum
-      float ls[4] = {0.f, 0.f, 0.f, 0.f};
-      uint32_t pk[32];
-#pragma unroll
-      for (int e = 0; e < 32; ++e) {  // ex2(-inf) = 0 for the hidden keys (m_use is finite)
-        const float p0 = ex2(__uint_as_float(sv[2 * e]) * p.scale_log2 - m_use);
-        const float p1 = ex2(__uint_as_float(sv[2 * e + 1]) * p.scale_log2 - m_use);
-        const __nv_bfloat162 b = __floats2bfloat162_rn(p0, p1);
-        // the row sum uses the bf16-rounded probabilities, i.e. exactly what the PV MMA consumes
-        ls[e & 3] += __bfloat162float(b.x) + __bfloat162float(b.y);
-        pk[e] = *reinterpret_cast<const uint32_t *>(&b);
-      }
-      const float l_tile = (ls[0] + ls[1]) + (ls[2] + ls[3]);
-      // P buffer (i & 1) is free: PV(i-2) completed before o_full(i-2), which this thread observed in iteration i-1
-      tmem_st32(tmem + lane_addr + ((i & 1) ? TM_P1 : TM_P0) + half * 32, pk);
-      tmem_st_wait();
-      l_run = l_run * alpha + l_tile;
-      m_run = m_new;
-      tc_fence_before();    // orders the tcgen05.ld of S and the tcgen05.st of P before the issuer's next MMAs
-      mbar_arrive(bar_p_full + 8 * (i & 1));
-      if (row == 0 && half == 0 && i == 0) DBG(7);
-      // fold the PREVIOUS tile's PV into the register accumulator (this half's 64 head-dim columns) while the tensor
-      // core works on PV(i) / QK(i+1): O(i-1) was computed against m_{i-1}, so the older sum is rescaled by
-      // alpha_{i-1} = 2^(m_{i-2} - m_{i-1})
-      if (i > 0) {
-        mbar_wait(bar_o_full, (i - 1) & 1);
-        tc_fence_after();
-        tmem_ld32(tmem + lane_addr + TM_O + half * 64, sv);
-        tmem_ld32(tmem + lane_addr + TM_O + half * 64 + 32, sv + 32);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(bar_o_free);
-#pragma unroll
-        for (int j = 0; j < 64; ++j) acc[j] = acc[j] * alpha_prev + __uint_as_float(sv[j]);
-      }
-      alpha_prev = alpha;
-    }
-    if (ntile > 0) {
-      mbar_wait(bar_o_full, (ntile - 1) & 1);
-      tc_fence_after();
-      if (row == 0 && half == 0) DBG(8);
-      tmem_ld32(tmem + lane_addr + TM_O + half * 64, sv);
-      tmem_ld32(tmem + lane_addr + TM_O + half * 64 + 32, sv + 32);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] = acc[j] * alpha_prev + __uint_as_float(sv[j]);
-      tc_fence_before();
-    }
-    if (row == 0 && half == 0) DBG(9);
-    // total row sum = both halves (same running max, so the partial sums just add)
-    {
-      float *xl = reinterpret_cast<float *>(sm + SMEM_XCH) + 512;
-      xl[half * 128 + row] = l_run;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      l_run += xl[(half ^ 1) * 128 + row];
-    }
-    if (ns == 1) {
-      // single split: normalise and write this half of the final bf16 row
-      if (row_live) {
-        const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-        uint4 *dst = reinterpret_cast<uint4 *>(p.out + ((row0 + node) * p.n_q_heads + hq0 + hs) * HD + half * 64);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          __nv_bfloat162 b0 = __floats2bfloat162_rn(acc[8 * j] * inv, acc[8 * j + 1] * inv);
-          __nv_bfloat162 b1 = __floats2bfloat162_rn(acc[8 * j + 2] * inv, acc[8 * j + 3] * inv);
-          __nv_bfloat162 b2 = __floats2bfloat162_rn(acc[8 * j + 4] * inv, acc[8 * j + 5] * inv);
-          __nv_bfloat162 b3 = __floats2bfloat162_rn(acc[8 * j + 6] * inv, acc[8 * j + 7] * inv);
-          dst[j] = make_uint4(*reinterpret_cast<uint32_t *>(&b0), *reinterpret_cast<uint32_t *>(&b1),
-                              *reinterpret_cast<uint32_t *>(&b2), *reinterpret_cast<uint32_t *>(&b3));
-        }
-      }
+      if (tid == 0) DBG(10);
     } else {
-      // several splits: the ns CTAs of this head group form one thread-block cluster.  After everyone has left its
-      // tile loop (barrier A: the Q/P/KV tiles of every CTA are dead) each thread pushes its row half - acc, and the
-      // row's (m, l) - straight into the shared memory of the CTA that owns that row's slice (DSMEM), barrier B,
-      // and every CTA combines its slice locally: no workspace round trip through L2, no serial last-arriver merge.
-      barrier_a();
-      if (row == 0 && half == 0) DBG(14);
-      const int RS = (rows_used + ns - 1) / ns;       // rows per owner CTA
-      const int owner = row / RS, rl = row % RS;
-      if (row_live) {
-        // partial rows are stored chunk-major ([32 float4 chunks][slot]) so that the lanes of a warp (= consecutive
-        // rows) write consecutive 16-byte words of the owner's buffer with every store instruction
-        const uint32_t dst = map_to_cta(base + mrg_acc + (uint32_t)((half * 16) * mrg_stride + split * RS + rl) * 16, owner);
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          st_cluster_f4(dst + (uint32_t)(j * mrg_stride) * 16, acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-        if (half == 0) st_cluster_f2(map_to_cta(base + mrg_ml + (uint32_t)(split * RS + rl) * 8, owner), m_run, l_run);
-      }
-      __syncwarp();  // the live-row branch above diverges; the cluster barrier is warp-aligned
-      if (row == 0 && half == 0) DBG(15);
-      cluster_sync_all();
+      if (ns > 1) { barrier_a(); cluster_sync_all(); }  // idle warpgroup (rows 64..127 of an MHA tile)
     }
-    if (row == 0 && half == 0) DBG(10);
-  } else {
-    if (ns > 1) { barrier_a(); cluster_sync_all(); }  // idle softmax warps (rows 64..127 of an MHA tile)
   }
   if (ns > 1) {
     // combine this CTA's row slice: out[r][:] = sum_i acc_i 2^(m_i - M) / sum_i l_i 2^(m_i - M), all operands local
@@ -670,8 +602,8 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
     const float2 *mml = reinterpret_cast<const float2 *>(sm + mrg_ml);
     const int items = RS * (HD / 4);
     // RS and np are powers of two in every configuration but ragged ones: shifts instead of four integer divisions per
-    // item, and all ns partials of an item are loaded before the first is used (the loop over a runtime ns was a chain
-    // of dependent shared-memory round trips: 1.7 us for 512 items on 320 threads)
+    // item, and all ns partials of an item are loaded before the first is used (a loop over a runtime ns would be a
+    // chain of dependent shared-memory round trips)
     const bool pow2 = (RS & (RS - 1)) == 0 && (p.np & (p.np - 1)) == 0;
     const int rs_sh = 31 - __clz(RS), np_sh = 31 - __clz(p.np);
     for (int it = tid; it < items; it += NTHREADS) {
@@ -705,15 +637,6 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
     }
   }
   if (tid == 0) DBG(12);
-  // every tcgen05 access of this CTA is complete (the softmax warps observed the last o_full): release TMEM
-  tc_fence_before();
-  __syncthreads();
-  if (tid == 0) DBG(13);
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS));
-  }
-  if (tid == 0) DBG(11);
 }
 
 }  // namespace attn
@@ -771,7 +694,7 @@ extern "C" int pia_attn_plan_create(const pia_attn_config_t *cfg, void *d_k_cach
   p->heads_per_cta = (cfg->max_nodes == 64 && G % 2 == 0) ? 2 : 1;
   p->n_groups = cfg->n_q_heads / p->heads_per_cta;
   p->mask_words = cfg->max_nodes / 64;
-  int n_sm = 148, dev = 0;
+  int n_sm = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   const int max_tiles = (cfg->max_seq + BN - 1) / BN;

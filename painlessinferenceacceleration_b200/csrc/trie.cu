@@ -1,4 +1,4 @@
-// GPU-resident trie draft cache for PIA LOOKAHEAD (sm_100a).
+// GPU-resident trie draft cache for PIA LOOKAHEAD (sm_90a).
 //
 // Takes over common/lookahead_cache.py of the reference (Tree :24-333, LookaheadCache :336-587): the
 // reference keeps one Python dict-of-dicts per first token; here the whole forest lives in HBM as

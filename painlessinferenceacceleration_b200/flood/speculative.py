@@ -1,7 +1,7 @@
 # -*- coding: utf-8 -*-
 """Drop-in for /root/reference/flood/flood/utils/speculative.py: `Spec` (:6-20) and `Lookahead(Spec)` (:23-124), the
 hash-table lookahead draft FLOOD's batcher drives (flood/utils/batch.py:484 lookahead_batching).  Same constructor,
-same four methods, same tensors in and out; the Triton kernels of flood/ops/draft.py are replaced by the sm_100a
+same four methods, same tensors in and out; the Triton kernels of flood/ops/draft.py are replaced by the sm_90a
 kernels of csrc/flood_draft.cu through the C ABI (include/pia_b200.h, pia_flood_*).  No CPU fallback."""
 import math
 import os

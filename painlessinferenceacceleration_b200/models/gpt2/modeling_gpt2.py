@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""GPT-2 with the lookahead patch, B200-native.
+"""GPT-2 with the lookahead patch, H100-native.
 
 Reference: /root/reference/lookahead/lookahead/models/gpt2/modeling_gpt2.py - patch :805-809 (rank-4 mask ->
 position_ids = rowsum - 1, additive mask), attention `_attn` :183-221 (its own causal bias AND the tree mask; a tree
@@ -7,7 +7,7 @@ mask is a subset of the causal one, so one visibility test suffices), Conv1D pro
 tied lm_head.  The module tree and parameter names are HF's (`transformer.wte/wpe/h.N.{ln_1,attn.c_attn,attn.c_proj,
 ln_2,mlp.c_fc,mlp.c_proj}/ln_f`), so checkpoints load unchanged.
 
-GPT-2's heads are 64 wide (any width <= 128 works): they run on the SAME tcgen05 tree-attention kernel as the Llama
+GPT-2's heads are 64 wide (any width <= 128 works): they run on the SAME wgmma tree-attention kernel as the Llama
 family by zero-padding every head to the kernel's 128-wide tile - the fused c_attn weight is re-laid out once so that
 the projection writes padded q | k | v heads, K/V are appended to the cache through k_rope_kv_append with an identity
 rotation table (cos = 1, sin = 0: GPT-2 has learned absolute positions, added to the embedding), the kernel's softmax
@@ -74,7 +74,7 @@ class GPT2LMHeadModel(LookaheadPreTrainedModel):
         super().__init__(config)
         if device is None:
             device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else 'meta'
-        assert dtype == torch.bfloat16, 'the B200 path computes in bf16'
+        assert dtype == torch.bfloat16, 'the H100 path computes in bf16'
         assert config.n_embd % config.n_head == 0 and config.n_embd // config.n_head <= PAD_D
         self.transformer = GPT2Model(config, device, dtype)
         self.lm_head = nn.Linear(config.n_embd, config.vocab_size, bias=False, device=device, dtype=dtype)

@@ -1,12 +1,12 @@
 # -*- coding: utf-8 -*-
-"""Llama with the lookahead patch, B200-native.
+"""Llama with the lookahead patch, H100-native.
 
 Reference: /root/reference/lookahead/lookahead/models/llama/modeling_llama.py
   patch :584-588 (rank-4 mask -> position_ids = rowsum-1, additive mask), attention :243-308, RoPE :93-169,
   RMSNorm :76-90, MLP :172-186, LM head :768-769.
 The module tree and parameter names are HF's (so checkpoints load unchanged); the forward over a draft of
 <= 64/128 tree nodes runs on static buffers:  fused QKV / gate-up cuBLAS GEMMs + libpia_b200 kernels
-(rmsnorm+residual, rope+kv-append into a preallocated cache, tcgen05 tree attention, silu*mul).  The rank-4 mask
+(rmsnorm+residual, rope+kv-append into a preallocated cache, wgmma tree attention, silu*mul).  The rank-4 mask
 is never built: `mask` is the per-node ancestor bit set, the prefix is implicit."""
 import glob
 import json
@@ -76,7 +76,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         super().__init__(config)
         if device is None:
             device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else 'meta'
-        assert dtype == torch.bfloat16, 'the B200 path computes in bf16'
+        assert dtype == torch.bfloat16, 'the H100 path computes in bf16'
         self.model = self.model_cls(config, device, dtype)
         self.lm_head = nn.Linear(config.hidden_size, config.vocab_size, bias=False, device=device, dtype=dtype)
         self._fused = False
@@ -185,7 +185,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
 
     # ------------------------------------------------------------------ weight-streaming GEMM plans (decode rows)
     def _gemm_plans(self, rt):
-        """tcgen05 weight-streaming GEMMs (csrc/gemm_ws.cu) for the 64-row decode buffers: HBM-tiled copies of the
+        """wgmma weight-streaming GEMMs (csrc/gemm_ws.cu) for the 64-row decode buffers: HBM-tiled copies of the
         fused weights, one plan per (weight, activation buffer).  Prefill passes (256 rows) stay on cuBLAS."""
         plans = getattr(rt, 'gemm_plans', None)
         if plans is not None:
@@ -207,14 +207,13 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         return plans
 
     def _layer_gemm_plans(self, layer, b):
-        """Which projections go through k_gemm_ws is decided by measurement (Llama-2-7B shapes; whole verify forward
-        as one CUDA graph, scripts/microbench.py --forward-only, us per forward): gate_up only 3453; + down as a
-        4-CTA cluster split-K (fp32 partials reduced through DSMEM) 3421; + o (cluster 4) 3527; + qkv (cluster 2)
-        3482; everything 3740 - a k_gemm_ws launched behind the 200 KB-per-SM attention kernel cannot use its early
-        weight streaming, and cuBLAS' 64x32 tiles win on the 32/96-tile projections.  Per launch (scripts/gemm_bench.py):
-        gate_up 31.5 us vs cuBLAS 34.6, lm_head 42.3 vs 46.6.  PIA_GEMM_SET overrides the set."""
+        """Which projections go through k_gemm_ws is decided by measurement (H100 80GB HBM3 SXM, 700 W; Llama-2-7B
+        shapes; whole verify forward as one CUDA graph, scripts/microbench.py --forward-only, us per forward): gate_up
+        only 6179; gate_up with the SiLU*up epilogue + down 6249; gate_up + down as a 4-CTA cluster split-K (fp32
+        partials reduced through DSMEM) 6353; + o (cluster 4) 6622; + qkv (cluster 2) 6795 - on the narrow
+        projections (32 / 96 weight tiles on 132 SMs) cuBLAS is faster.  PIA_GEMM_SET overrides the set."""
         import os
-        want = os.environ.get('PIA_GEMM_SET', 'gate_up,down').split(',')
+        want = os.environ.get('PIA_GEMM_SET', 'gate_up').split(',')
         plans = {}
         if 'gate_up_silu' in want and layer.mlp.gate_up_weight.shape[0] % 256 == 0:
             # SiLU(gate) * up in the GEMM epilogue: every 128-row weight tile holds 64 gate rows + the 64 up rows of the same

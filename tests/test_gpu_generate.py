@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""End-to-end parity of the B200 loop (generate -> lookahead_generation, one CUDA graph per step) with the CPU
+"""End-to-end parity of the H100 loop (generate -> lookahead_generation, one CUDA graph per step) with the CPU
 restatement of the reference loop (oracle/loop.py) on seeded tiny models that share their weights.
 
 bf16 caveat (lookahead/README.md:45, SURVEY A.2-16): identical text is only guaranteed in fp32; in bf16 the two
@@ -298,7 +298,7 @@ def _shape_model(name, layers=None):
 @pytest.mark.big
 @pytest.mark.parametrize('name,layers,penalty,n_prompts,new', [('llama2-7b', None, 1.0, 4, 128),
                                                                ('mistral-7b', None, 1.1, 3, 96),
-                                                               ('mixtral-8x7b', 3, 1.0, 3, 64)])
+                                                               ('mixtral-8x7b-16l', 3, 1.0, 3, 64)])
 def test_loop_is_exact_at_baseline_shapes(name, layers, penalty, n_prompts, new):
     """Llama-2-7B (32 layers, 4096, MHA-32, V=32000; config 2), Mistral-7B (GQA-4) with repetition_penalty=1.1
     (config 3) and an 8-expert Mixtral-8x7B-shaped slice (3 of the 32 layers; config 4): the oracle loop (reference
@@ -391,7 +391,7 @@ def _gpt2_pair(seed):
 
 def test_gpt2_verify_logits_and_loop():
     """GPT-2 (64-wide or narrower heads, learned positions, LayerNorm, gelu_new, Conv1D + bias, tied head) through the
-    shared kernels: heads zero-padded to the 128-wide tcgen05 attention tile.  (i) logits vs an fp32 evaluation of the
+    shared kernels: heads zero-padded to the 128-wide attention tile.  (i) logits vs an fp32 evaluation of the
     same weights within 2 x the eager bf16 model's own error + 0.02; (ii) the oracle loop (reference semantics, 16-token
     / 4-branch drafts = BASELINE config 1) driving one copy == our fused device loop on the other copy: tokens, dls,
     edls identical; (iii) lookahead == plain greedy on the same kernels."""

@@ -528,7 +528,7 @@ def test_moe_router():
 @pytest.mark.parametrize('N,K,split', [(256, 128, 1), (12288, 4096, 1), (4096, 4096, 4), (22016, 4096, 1),
                                        (4096, 11008, 4), (32000, 4096, 1), (4096, 4096, 1), (1024, 14336, 7)])
 def test_gemm_weight_streaming(N, K, split):
-    """tcgen05 weight-streaming GEMM vs an fp32 matmul of the same bf16 operands (nn.Linear semantics,
+    """wgmma weight-streaming GEMM vs an fp32 matmul of the same bf16 operands (nn.Linear semantics,
     modeling_llama.py:254-256/:303/:185-186/:769).  Tolerance: one bf16 rounding of the fp32 result."""
     from painlessinferenceacceleration_b200.common import ops
     torch.manual_seed(N + K)

@@ -1,6 +1,7 @@
 # -*- coding: utf-8 -*-
 """Host-side logic that needs no GPU: generation-mode selection, kwargs validation, bench sharding over a
 world_size-2 gloo group (the N>1 path is independent replicas + one weight broadcast)."""
+import json
 import os
 import subprocess
 import sys
@@ -118,14 +119,17 @@ def test_reference_arm_under_torchrun_prints_one_line_from_rank0():
     assert d['mean_accepted_len_per_step'] >= 1.0
 
 
-def test_bench_helpers_traffic_lookup_and_synthetic_weights():
-    """bench.py host helpers: roofline.traffic comes from the newest committed ncu summary whose capture name and
-    kernel match; the synthetic weights are a pure function of (name, index) - the GPU arm and the CPU arms build the
-    same model - and make greedy decoding follow the successor chain when the embedding dominates"""
+def test_bench_helpers_traffic_lookup_and_synthetic_weights(tmp_path):
+    """bench.py host helpers: roofline.traffic comes from the newest ncu summary whose capture name and kernel match;
+    the synthetic weights are a pure function of (name, index) - the GPU arm and the CPU arms build the same model -
+    and make greedy decoding follow the successor chain when the embedding dominates"""
     import bench
-    t = bench.ncu_traffic('prof_attn_short', 'k_tree_attn')
-    assert t is not None and 1e6 < t < 1e9
-    assert bench.ncu_traffic('no_such_capture', 'k_tree_attn') is None
+    (tmp_path / 'r01_traffic.json').write_text(json.dumps({'prof_attn_short_r1:k_tree_attn': 5e6}))
+    (tmp_path / 'r02_traffic.json').write_text(json.dumps({'prof_attn_short_r2:k_tree_attn': 9e6,
+                                                           'prof_gemm_ws_r2:k_gemm_ws<4>': 1.8e8}))
+    t = bench.ncu_traffic('prof_attn_short', 'k_tree_attn', str(tmp_path))
+    assert t is not None and 1e6 < t < 1e9 and t == 9e6
+    assert bench.ncu_traffic('no_such_capture', 'k_tree_attn', str(tmp_path)) is None
     hbm, tf, src = bench.peaks()
     assert hbm > 1000 and tf > 100 and src in ('measured', 'fallback')
     a = bench.hashed_normal_(torch.empty((3, 1 << 16), dtype=torch.bfloat16), 77, 0.02)
