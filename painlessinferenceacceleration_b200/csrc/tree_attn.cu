@@ -6,8 +6,9 @@
 // The mask is never materialised: prefix keys [pad_len, P) are visible to every row, the n draft keys follow the
 // row's ancestor bit set (uint64 words, produced by the trie kernel) held in registers.
 //
-// One CTA = (KV split, head group).  A head group is one KV head's worth of rows packed into a single 128-row
-// tile: 2 query heads x 64 draft rows under GQA, 1 head otherwise (rows 64..127 idle for MHA/64).
+// One CTA = (KV split, head group).  A head group is up to two query heads of ONE KV head packed into a single 128-row
+// tile: at 64 draft rows the G = Hq / Hkv query heads of a KV head fill ceil(G / 2) tiles of 2 heads, the last tile
+// holding 1 head when G is odd (and the only one under MHA: rows 64..127 idle); at 128 draft rows 1 head per tile.
 // Warp roles (288 threads):  warps 0-7 = two consumer warpgroups, each owning 64 rows (wgmma M = 64): they stage Q
 //                            (and, fused, the draft tile), issue the MMAs and run the softmax in registers,
 //                            warp 8 = TMA producer (K/V tiles of 128 keys, 2-stage ring, V on its own barriers).
@@ -166,6 +167,7 @@ struct Params {
   int slot_planes;         // KV planes between consecutive slots' caches (0: shared cache)
   int plane0;              // first plane of the cache slot 0 addresses
   int layer, n_q_heads, n_kv_heads, np, mask_words, heads_per_cta, max_seq, n_split, tiles_per_cta;
+  int ctas_per_kv;         // head groups per KV head: ceil(G / heads_per_cta); heads_per_cta = 2 at 64 draft rows, 1 at 128
   float scale_log2;
   // fused mode (pia_tree_attn_fused_fwd): RoPE + KV append happen here.  Q and the draft nodes' K / V come straight from
   // the fused projection output, the draft keys are one extra tile built in shared memory, the cache only holds [0, P)
@@ -183,6 +185,19 @@ __device__ __forceinline__ unsigned long long gtime() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+// head group (blockIdx.y) -> KV head hkv, its j-th tile of query heads, first query head hq0 and heads in the tile:
+// the G query heads of a KV head fill ceil(G / heads_per_cta) tiles, the last one holding a single head when G is odd
+struct HeadGroup { int hkv, j, hq0, heads; };
+__device__ __forceinline__ HeadGroup head_group(const Params &p, int group) {
+  const int G = p.n_q_heads / p.n_kv_heads;
+  HeadGroup g;
+  g.hkv = group / p.ctas_per_kv;
+  g.j = group - g.hkv * p.ctas_per_kv;
+  g.hq0 = g.hkv * G + g.j * p.heads_per_cta;
+  g.heads = min(p.heads_per_cta, G - g.j * p.heads_per_cta);
+  return g;
+}
+
 #define DBG(ev) do { if (p.dbg) p.dbg[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 16 + (ev)] = gtime(); } while (0)
 
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -214,8 +229,8 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
   if (n <= 0) return;      // idle slot: every CTA of its clusters takes this exit
   const long long row0 = (long long)slot * p.sl.rows_per_slot;  // first activation / mask row of the slot
   const int L = P + n;
-  const int hq0 = group * p.heads_per_cta;
-  const int hkv = hq0 / (p.n_q_heads / p.n_kv_heads);
+  const HeadGroup hg = head_group(p, group);
+  const int hkv = hg.hkv, hq0 = hg.hq0, heads_here = hg.heads;
   // tiles: plain mode = the keys [0, L) of the cache; fused mode = the prefix tiles [0, P) of the cache + ONE draft tile
   // (the n draft keys, rotated and staged in shared memory by the consumer warps of the CTA that owns the last tile)
   const bool fused = p.fused != 0;
@@ -223,7 +238,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
   const int tiles_total = fused ? Tp + 1 : (L + BN - 1) / BN;
   // Work split decided on the device from the live length: tiles_per_cta tiles per CTA (more only when the
   // plan's split limit is reached); a single split writes the final output directly (no partials, no merge).
-  const int rows_used = p.heads_per_cta * p.np;          // 64 (MHA, 64 nodes) or 128
+  const int rows_used = heads_here * p.np;               // 64 (one head of 64 nodes) or 128
   const int n_wg = rows_used / 64;                       // consumer warpgroups with live rows
   const bool ded = (rows_used + MAX_SPLIT) * HD * 4 <= MRG_DED_ACC_BYTES;
   int ns = (tiles_total + p.tiles_per_cta - 1) / p.tiles_per_cta;
@@ -305,7 +320,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
       if (srow < rows_used) {
         if (!fused) {
           uint4 qv[8];  // Q row -> shared memory (K-major SWIZZLE_128B); each half loads one 64-wide d sub-tile
-          const bool have = hs < p.heads_per_cta && node < n;
+          const bool have = hs < heads_here && node < n;
           const uint4 *src = reinterpret_cast<const uint4 *>(p.q + ((row0 + node) * p.n_q_heads + hq0 + hs) * HD) + half * 8;
 #pragma unroll
           for (int ch = 0; ch < 8; ++ch) qv[ch] = have ? src[ch] : make_uint4(0, 0, 0, 0);
@@ -325,7 +340,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
           const uint4 *sn = reinterpret_cast<const uint4 *>(p.sin_t + (long long)pos * (HD / 2));
           const long long row_elems = (long long)(p.n_q_heads + 2 * p.n_kv_heads) * HD;
           const __nv_bfloat16 *xr = p.qkv + (row0 + node) * row_elems;
-          const bool have = hs < p.heads_per_cta && node < n;
+          const bool have = hs < heads_here && node < n;
           // All global loads of a batch are issued (read-only path: the compiler may not move plain loads across the
           // shared memory stores in between, and eight dependent load rounds would serialise the prologue) before the
           // first value is used; four 16-byte chunks per batch bound the registers.
@@ -354,7 +369,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
             // rows; one CTA per KV head also appends the rows to the cache for the steps to come (pretrained_model.py:
             // the reference's torch.cat of past and new K/V, modeling_llama.py:265-268)
             const bool key_row = hs == 0 && node < n;
-            const bool writer = (hq0 % (p.n_q_heads / p.n_kv_heads)) == 0;
+            const bool writer = hg.j == 0;  // the first head group of the KV head (hq0 % G == 0)
             const uint4 *ka = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + half * 8;
             const uint4 *kb = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + (half ^ 1) * 8;
             const uint4 *va = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + p.n_kv_heads + hkv) * HD) + half * 8;
@@ -544,6 +559,8 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         if (lane == 0) mbar_arrive(bar_kv_empty + 8 * s);  // this warp is done with the stage's K and V
       }
       if (tid == 0) DBG(8);
+      // derived again from blockIdx.y rather than held through the tile loop (holding it there adds register spills)
+      const HeadGroup hl = head_group(p, group);
       // total row sum = the four lanes of the row (same running max, so the partial sums just add)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -557,7 +574,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         for (int h = 0; h < 2; ++h) {
           if (live[h]) {
             const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
-            uint32_t *dst = reinterpret_cast<uint32_t *>(p.out + ((row0 + node[h]) * p.n_q_heads + hq0 + hs[h]) * HD);
+            uint32_t *dst = reinterpret_cast<uint32_t *>(p.out + ((row0 + node[h]) * p.n_q_heads + hl.hq0 + hs[h]) * HD);
 #pragma unroll
             for (int nb = 0; nb < 16; ++nb) {
               __nv_bfloat162 b = __floats2bfloat162_rn(o[4 * nb + 2 * h] * inv, o[4 * nb + 2 * h + 1] * inv);
@@ -572,7 +589,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         // and every CTA combines its slice locally: no workspace round trip through L2, no serial last-arriver merge.
         barrier_a();
         if (tid == 0) DBG(14);
-        const int RS = (rows_used + ns - 1) / ns;       // rows per owner CTA
+        const int RS = (hl.heads * p.np + ns - 1) / ns;  // rows per owner CTA
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (live[h]) {
@@ -592,12 +609,14 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
       }
       if (tid == 0) DBG(10);
     } else {
-      if (ns > 1) { barrier_a(); cluster_sync_all(); }  // idle warpgroup (rows 64..127 of an MHA tile)
+      if (ns > 1) { barrier_a(); cluster_sync_all(); }  // idle warpgroup (rows 64..127 of a one-head tile)
     }
   }
   if (ns > 1) {
     // combine this CTA's row slice: out[r][:] = sum_i acc_i 2^(m_i - M) / sum_i l_i 2^(m_i - M), all operands local
-    const int RS = (rows_used + ns - 1) / ns;
+    const HeadGroup hl = head_group(p, group);  // derived again (see above)
+    const int rows_late = hl.heads * p.np;
+    const int RS = (rows_late + ns - 1) / ns;
     const float4 *macc = reinterpret_cast<const float4 *>(sm + mrg_acc);
     const float2 *mml = reinterpret_cast<const float2 *>(sm + mrg_ml);
     const int items = RS * (HD / 4);
@@ -609,7 +628,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
     for (int it = tid; it < items; it += NTHREADS) {
       const int rl = pow2 ? (it & (RS - 1)) : it % RS, c4 = pow2 ? (it >> rs_sh) : it / RS;
       const int r = split * RS + rl;
-      if (r >= rows_used) continue;
+      if (r >= rows_late) continue;
       const int rh = pow2 ? (r >> np_sh) : r / p.np, rn = pow2 ? (r & (p.np - 1)) : r % p.np;
       if (rn >= n) continue;
       float2 ml[MAX_SPLIT];
@@ -632,7 +651,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
       }
       const float inv = den > 0.f ? 1.f / den : 0.f;
       __nv_bfloat162 b0 = __floats2bfloat162_rn(o4.x * inv, o4.y * inv), b1 = __floats2bfloat162_rn(o4.z * inv, o4.w * inv);
-      reinterpret_cast<uint2 *>(p.out + ((row0 + rn) * p.n_q_heads + hq0 + rh) * HD)[c4] =
+      reinterpret_cast<uint2 *>(p.out + ((row0 + rn) * p.n_q_heads + hl.hq0 + rh) * HD)[c4] =
           make_uint2(*reinterpret_cast<uint32_t *>(&b0), *reinterpret_cast<uint32_t *>(&b1));
     }
   }
@@ -649,7 +668,7 @@ using namespace pia::attn;
 struct pia_attn_plan {
   pia_attn_config_t cfg;
   CUtensorMap map_k, map_v;
-  int heads_per_cta, n_groups, n_split, mask_words, tiles_per_cta;
+  int heads_per_cta, ctas_per_kv, n_groups, n_split, mask_words, tiles_per_cta;
   unsigned long long *dbg;
   __nv_bfloat16 *k_base, *v_base;  // the caches the TMA maps describe (fused mode appends the draft rows itself)
 };
@@ -691,8 +710,11 @@ extern "C" int pia_attn_plan_create(const pia_attn_config_t *cfg, void *d_k_cach
   PIA_REQUIRE(p, "out of host memory");
   p->cfg = *cfg;
   const int G = cfg->n_q_heads / cfg->n_kv_heads;
-  p->heads_per_cta = (cfg->max_nodes == 64 && G % 2 == 0) ? 2 : 1;
-  p->n_groups = cfg->n_q_heads / p->heads_per_cta;
+  // two query heads of one KV head per 128-row tile at 64 draft rows (any G: an odd G leaves one head in its KV head's
+  // last tile), one head at 128 draft rows
+  p->heads_per_cta = cfg->max_nodes == 64 ? 2 : 1;
+  p->ctas_per_kv = (G + p->heads_per_cta - 1) / p->heads_per_cta;
+  p->n_groups = cfg->n_kv_heads * p->ctas_per_kv;
   p->mask_words = cfg->max_nodes / 64;
   int n_sm = 132, dev = 0;
   cudaGetDevice(&dev);
@@ -761,7 +783,8 @@ static int attn_launch(pia_attn_plan_t *p, int layer, const void *d_q, const voi
   a.slot_planes = slots->kv_slot_stride ? p->cfg.n_layers * p->cfg.n_kv_heads : 0;
   a.plane0 = slots->kv_first_slot * p->cfg.n_layers * p->cfg.n_kv_heads;
   a.layer = layer; a.n_q_heads = p->cfg.n_q_heads; a.n_kv_heads = p->cfg.n_kv_heads; a.np = p->cfg.max_nodes;
-  a.mask_words = p->mask_words; a.heads_per_cta = p->heads_per_cta; a.max_seq = p->cfg.max_seq;
+  a.mask_words = p->mask_words; a.max_seq = p->cfg.max_seq;
+  a.heads_per_cta = p->heads_per_cta; a.ctas_per_kv = p->ctas_per_kv;
   // KV splits per (slot, head group): one wave of CTAs over ALL slots - a batch of requests brings its own parallelism,
   // so each cluster shrinks (8 slots x 32 head groups already cover the SMs without any split)
   int ns = p->n_split / slots->batch;

@@ -27,14 +27,15 @@ class LlamaRMSNorm(nn.Module):
 
 
 class LlamaAttention(nn.Module):
-    def __init__(self, cfg, device, dtype):
+    def __init__(self, cfg, device, dtype, qkv_bias=False):
         super().__init__()
         hd = cfg.hidden_size // cfg.num_attention_heads
         kv = getattr(cfg, 'num_key_value_heads', None) or cfg.num_attention_heads
         kw = dict(bias=False, device=device, dtype=dtype)
-        self.q_proj = nn.Linear(cfg.hidden_size, cfg.num_attention_heads * hd, **kw)
-        self.k_proj = nn.Linear(cfg.hidden_size, kv * hd, **kw)
-        self.v_proj = nn.Linear(cfg.hidden_size, kv * hd, **kw)
+        qkw = dict(kw, bias=qkv_bias)
+        self.q_proj = nn.Linear(cfg.hidden_size, cfg.num_attention_heads * hd, **qkw)
+        self.k_proj = nn.Linear(cfg.hidden_size, kv * hd, **qkw)
+        self.v_proj = nn.Linear(cfg.hidden_size, kv * hd, **qkw)
         self.o_proj = nn.Linear(cfg.num_attention_heads * hd, cfg.hidden_size, **kw)
 
 
@@ -48,9 +49,11 @@ class LlamaMLP(nn.Module):
 
 
 class LlamaDecoderLayer(nn.Module):
+    qkv_bias = False   # biases on q/k/v (Qwen2); o_proj never has one
+
     def __init__(self, cfg, device, dtype):
         super().__init__()
-        self.self_attn = LlamaAttention(cfg, device, dtype)
+        self.self_attn = LlamaAttention(cfg, device, dtype, qkv_bias=self.qkv_bias)
         self.mlp = self._make_mlp(cfg, device, dtype)
         self.input_layernorm = LlamaRMSNorm(cfg.hidden_size, cfg.rms_norm_eps, device, dtype)
         self.post_attention_layernorm = LlamaRMSNorm(cfg.hidden_size, cfg.rms_norm_eps, device, dtype)
@@ -130,7 +133,8 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         return sd
 
     def fuse(self):
-        """QKV and gate/up weights into single GEMM operands; the HF-named parameters become views of them"""
+        """QKV and gate/up weights (and the QKV biases, if any) into single GEMM operands; the HF-named parameters
+        become views of them"""
         if self._fused:
             return
         for layer in self.model.layers:
@@ -139,6 +143,11 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             nq, nk = a.q_proj.weight.shape[0], a.k_proj.weight.shape[0]
             a.q_proj.weight.data, a.k_proj.weight.data, a.v_proj.weight.data = w[:nq], w[nq:nq + nk], w[nq + nk:]
             a.qkv_weight = w
+            a.qkv_bias = None
+            if a.q_proj.bias is not None:
+                bias = torch.cat([a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data]).contiguous()
+                a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data = bias[:nq], bias[nq:nq + nk], bias[nq + nk:]
+                a.qkv_bias = bias
             self._fuse_mlp(layer)
         self._fused = True
 
@@ -214,6 +223,8 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         projections (32 / 96 weight tiles on 132 SMs) cuBLAS is faster.  PIA_GEMM_SET overrides the set."""
         import os
         want = os.environ.get('PIA_GEMM_SET', 'gate_up').split(',')
+        if ('qkv' in want or 'qkv2' in want) and layer.self_attn.qkv_bias is not None:
+            raise ValueError('PIA_GEMM_SET names qkv, but this model has QKV biases and k_gemm_ws has no bias epilogue')
         plans = {}
         if 'gate_up_silu' in want and layer.mlp.gate_up_weight.shape[0] % 256 == 0:
             # SiLU(gate) * up in the GEMM epilogue: every 128-row weight tile holds 64 gate rows + the 64 up rows of the same
@@ -341,6 +352,8 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             a = layer.self_attn
             if lp and 'qkv' in lp:
                 lp['qkv'].run(64, out=b.qkv)
+            elif a.qkv_bias is not None:   # bias added in fp32 before the one bf16 rounding, as F.linear does
+                torch.addmm(a.qkv_bias, b.y, a.qkv_weight.t(), out=b.qkv)
             else:
                 torch.mm(b.y, a.qkv_weight.t(), out=b.qkv)
             if pf and lp and 'gate_up' in lp:
