@@ -256,6 +256,20 @@ int pia_gemm_plan_set_silu(pia_gemm_plan_t *g, int on);
 /* splits == 1: d_out is bf16 [rows_cap, N]; splits > 1: d_out is fp32 [splits][64][N] partial slices (sum them in
  * slice order, e.g. with pia_rmsnorm_partials).  rows <= 64 rows are written. */
 int pia_gemm_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream);
+/* FP8 (e4m3) weight-only variant of the same projections (modeling_llama.py:254-256, :303, :185-186; the experts of
+ * mixtral/modeling_mixtral.py:668-683): Y[t, n] = s[n] * sum_k X[t, k] q[n, k] (+ bias[n]), fp32 accumulate, one bf16
+ * rounding; q is symmetric e4m3 per weight row with fp32 scale s[n] (d_scale, [N] floats).  d_w holds q tiled as
+ * [N/128][K/128] contiguous blocks of 128 rows x 128 bytes, each 16-byte k group stored as k {0,1,8,9,2,3,10,11,4,5,12,
+ * 13,6,7,14,15} (ops.tile_weight_fp8).  N % 128 == 0, K % 128 == 0.  d_bias: [N] fp32 or NULL (the biased QKV of
+ * Qwen2, qwen2/modeling_qwen2.py); needs split_k == 1 or a cluster split.  split_k as for pia_gemm_plan_create, except
+ * that there is no stream-K (-1).  pia_gemm_run takes 1 <= rows <= x_rows; beyond 64 rows every 64-row block of X
+ * streams the weight again.  fp32 slices (split_k > 1) are [splits][x_rows][N].  set_silu / set_pdl / splits apply. */
+int pia_gemm_plan_create_fp8(const void *d_w, const void *d_scale, const void *d_bias, int N, int K, const void *d_x,
+                             int x_rows, int split_k, pia_gemm_plan_t **out);
+/* Grouped twin (MoE experts, mixtral/modeling_mixtral.py:692-759): d_w = `groups` tiled fp8 weights back to back,
+ * d_scale [groups * N]; out[g] ([x_rows, N] bf16, consecutive) = X[:, g*K : (g+1)*K] @ W[g]^T. */
+int pia_gemm_plan_create_grouped_fp8(const void *d_w, const void *d_scale, int groups, int N, int K, const void *d_x,
+                                     int x_rows, pia_gemm_plan_t **out);
 
 /* ============================================================================================
  * Fused elementwise pieces of the verify forward (all bf16 I/O, fp32 math)

@@ -51,6 +51,52 @@ def interleave_gate_up(w_gate_up):
     return torch.cat([g, u], dim=1).reshape(two_i, K).contiguous()
 
 
+FP8_MAX = 448.0
+# position p of every 16-byte k group of a tiled fp8 weight holds k = _FP8_KPERM[p]: thread c of a wgmma A fragment
+# finds its codes for k {2c, 2c+1} and {2c+8, 2c+9} in one 32-bit word
+_FP8_KPERM = (0, 1, 8, 9, 2, 3, 10, 11, 4, 5, 12, 13, 6, 7, 14, 15)
+
+
+def quantize_fp8(w):
+    """per-output-row symmetric e4m3 of a weight [..., N, K]: s[n] = amax(|W[n, :]|) / 448 (1 for an all-zero row),
+    q = RNE(clamp(W / s, +-448)); the dequantised weight is float(q) * s[n].  Returns (q float8_e4m3fn, s fp32 [..., N]);
+    computed in fp32 on w's device, a slab of rows at a time."""
+    q = torch.empty(w.shape, dtype=torch.float8_e4m3fn, device=w.device)
+    s = torch.empty(w.shape[:-1], dtype=torch.float32, device=w.device)
+    w2, q2, s2 = w.reshape(-1, w.shape[-1]), q.view(-1, w.shape[-1]), s.view(-1)
+    step = max(1, (1 << 26) // max(w.shape[-1], 1))
+    for r in range(0, w2.shape[0], step):
+        x = w2[r:r + step].float()
+        amax = x.abs().amax(dim=1)
+        sc = torch.where(amax > 0, amax / FP8_MAX, torch.ones_like(amax))
+        q2[r:r + step] = (x / sc[:, None]).clamp_(-FP8_MAX, FP8_MAX).to(torch.float8_e4m3fn)
+        s2[r:r + step] = sc
+    return q, s
+
+
+def tile_weight_fp8(q):
+    """e4m3 [..., N, K] -> uint8 [..., N/128, K/128, 128, 128] contiguous (the fp8 GEMM's HBM layout): one 16 KB block
+    per (128-row tile, 128-wide k chunk), k permuted inside every 16-byte group by _FP8_KPERM"""
+    N, K = q.shape[-2:]
+    if N % 128 or K % 128:
+        raise ValueError(f'the fp8 GEMM needs both weight dimensions to be multiples of 128, got [{N}, {K}]')
+    lead = q.shape[:-2]
+    b = q.view(torch.uint8).reshape(-1, N // 128, 128, K // 128, 8, 16)
+    perm = torch.tensor(_FP8_KPERM, device=q.device)
+    t = b.index_select(5, perm).permute(0, 1, 3, 2, 4, 5).reshape(*lead, N // 128, K // 128, 128, 128).contiguous()
+    return t
+
+
+def untile_weight_fp8(t):
+    """inverse of tile_weight_fp8: uint8 [..., N/128, K/128, 128, 128] -> e4m3 [..., N, K]"""
+    nt, kt = t.shape[-4:-2]
+    lead = t.shape[:-4]
+    inv = torch.empty(16, dtype=torch.long)
+    inv[torch.tensor(_FP8_KPERM)] = torch.arange(16)
+    b = t.reshape(-1, nt, kt, 128, 8, 16).index_select(5, inv.to(t.device))
+    return b.permute(0, 1, 3, 2, 4, 5).reshape(*lead, nt * 128, kt * 128).contiguous().view(torch.float8_e4m3fn)
+
+
 class Gemm(object):
     """pia_gemm_plan_t: Y = X @ W^T for one (weight, activation buffer) pair; `out` is bf16 [rows, N] when the plan
     has one K split, else fp32 [splits, 64, N]"""
@@ -86,6 +132,50 @@ class Gemm(object):
             L.check(self.lib.pia_gemm_plan_create_grouped(_p(weight), G, N, K, _p(x), x.shape[0], C.byref(self.h)))
         self.splits, self.N, self.weight, self._keep = 1, N, weight, (weight, x)
         self.out = torch.empty((G, 64, N), dtype=torch.bfloat16, device=weight.device)
+        return self
+
+    @classmethod
+    def fp8(cls, qweight, scale, x, bias=None, split_k=1, out=None):
+        """fp8 weight plan (pia_gemm_plan_create_fp8): qweight = tile_weight_fp8(q) of an [N, K] weight, scale fp32 [N]
+        (same row order), bias fp32 [N] or None; runs 1..x.shape[0] rows.  out (allocated unless given): bf16
+        [x_rows, N] (N/2 columns with set_silu), or fp32 [splits, x_rows, N] slices for split_k > 1"""
+        nt, kt = qweight.shape[-4:-2]
+        N, K = nt * 128, kt * 128
+        assert qweight.dtype == torch.uint8 and qweight.is_contiguous() and qweight.dim() == 4
+        assert scale.dtype == torch.float32 and scale.numel() == N and x.shape[1] == K and x.is_contiguous()
+        assert bias is None or (bias.dtype == torch.float32 and bias.numel() == N and bias.is_contiguous())
+        self = cls.__new__(cls)
+        self.lib = L.load()
+        self.h = L.vp()
+        with torch.cuda.device(qweight.device):
+            L.check(self.lib.pia_gemm_plan_create_fp8(_p(qweight), _p(scale), _p(bias), N, K, _p(x), x.shape[0],
+                                                      split_k, C.byref(self.h)))
+        self.splits = self.lib.pia_gemm_plan_splits(self.h)
+        self.N, self.weight, self._keep = N, qweight, (qweight, scale, bias, x)
+        if out is not None:
+            self.out = out
+        elif self.splits == 1:
+            self.out = torch.empty((x.shape[0], N), dtype=torch.bfloat16, device=x.device)
+        else:
+            self.out = torch.empty((self.splits, x.shape[0], N), dtype=torch.float32, device=x.device)
+        return self
+
+    @classmethod
+    def grouped_fp8(cls, qweight, scale, x):
+        """one launch for all experts (pia_gemm_plan_create_grouped_fp8): qweight = tile_weight_fp8 of [G, N, K],
+        scale fp32 [G, N], x [rows, G * K]; out bf16 [G, x_rows, N]"""
+        G, nt, kt = qweight.shape[:3]
+        N, K = nt * 128, kt * 128
+        assert qweight.dtype == torch.uint8 and qweight.is_contiguous() and qweight.dim() == 5
+        assert scale.dtype == torch.float32 and scale.numel() == G * N and x.shape[1] == G * K and x.is_contiguous()
+        self = cls.__new__(cls)
+        self.lib = L.load()
+        self.h = L.vp()
+        with torch.cuda.device(qweight.device):
+            L.check(self.lib.pia_gemm_plan_create_grouped_fp8(_p(qweight), _p(scale), G, N, K, _p(x), x.shape[0],
+                                                              C.byref(self.h)))
+        self.splits, self.N, self.weight, self._keep = 1, N, qweight, (qweight, scale, x)
+        self.out = torch.empty((G, x.shape[0], N), dtype=torch.bfloat16, device=x.device)
         return self
 
     def set_pdl(self, on=True):

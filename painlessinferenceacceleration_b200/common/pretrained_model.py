@@ -223,6 +223,10 @@ class LookaheadPreTrainedModel(nn.Module):
                 self._gemm_plans(rt)
         return rt
 
+    def quantize_fp8(self):
+        """fp8 weight-only mode; the Llama family implements it (GPT-2's linears run through torch)"""
+        raise NotImplementedError(f'{type(self).__name__} has no fp8 weight mode')
+
     def _decoding_args(self):
         return ['decoding_kwargs']
 

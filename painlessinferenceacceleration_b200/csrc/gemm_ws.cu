@@ -16,6 +16,7 @@
 //     partial slices that the consumer (k_rmsnorm_partials) sums in a fixed order - deterministic, no atomics.
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include <new>
 
@@ -468,6 +469,255 @@ k_gemm_sk(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
   }
 }
 
+// ------------------------------------------------------------------------------------------------ fp8 (e4m3) weights
+// W8A16: every weight row n is symmetric e4m3 with an fp32 scale s[n]; X stays bf16.  Same structure as k_gemm_ws
+// (swap-AB, two consumer warpgroups x wgmma M = 64, TMA producer warp over the mbarrier ring, HBM-tiled weight), but a
+// stage covers 128 k: one 16 KB weight block of 128 rows x 128 e4m3 bytes (one SWIZZLE_128B row per weight row) plus
+// the two matching 64-k bf16 X boxes.  The consumers read their wgmma A fragment straight from the staged fp8 bytes,
+// convert it to bf16 pairs in registers (exact: every finite e4m3 value is a bf16 value) and issue
+// wgmma.m64n64k16 with A in registers and X from shared memory.  Epilogue: y = acc * s[n] (+ bias[n]) in fp32, one bf16
+// rounding.  Row counts above 64: gridDim.z also runs over 64-row token blocks, each streaming the weight again.
+constexpr int F8_BK = 128;                                // k per stage: 128 e4m3 bytes = one 128-byte swizzle row
+constexpr int F8_W_BYTES = BMW * F8_BK;                   // 16 KB
+constexpr int F8_STAGE_BYTES = F8_W_BYTES + 2 * X_BYTES;  // + two 64-k bf16 X boxes
+constexpr int f8_smem_total(int nstage) { return nstage * F8_STAGE_BYTES + 256 + XCH_BYTES + 1024; }
+static_assert(ACC_OFF + BMW * ACC_LD * 4 <= 3 * F8_STAGE_BYTES, "accumulator staging must fit in the pipeline stages");
+
+// two e4m3 codes (low byte = lower k) -> bf16x2 (low half = lower k): e4m3 -> f16 is exact, f16 -> f32 -> bf16 too
+__device__ __forceinline__ void e4m3x4_to_bf16x2(uint32_t w, uint32_t &lo, uint32_t &hi) {
+  uint32_t h0, h1;
+  asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %0, l;\n\tcvt.rn.f16x2.e4m3x2 %1, h;\n\t}"
+      : "=r"(h0), "=r"(h1) : "r"(w));
+  const float2 f0 = __half22float2(*reinterpret_cast<const __half2 *>(&h0));
+  const float2 f1 = __half22float2(*reinterpret_cast<const __half2 *>(&h1));
+  const __nv_bfloat162 b0 = __floats2bfloat162_rn(f0.x, f0.y), b1 = __floats2bfloat162_rn(f1.x, f1.y);
+  lo = *reinterpret_cast<const uint32_t *>(&b0);
+  hi = *reinterpret_cast<const uint32_t *>(&b1);
+}
+// D[64 x 64] += A[64 x 16] * B[64 x 16]^T, A = bf16 pairs in registers, B K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n64k16_ra(float (&d)[32], const uint32_t *a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b)
+      : "memory");
+}
+
+struct F8Params {
+  int N, n_chunks, chunks_per_split, n_split, rows, ntb;  // n_chunks: K / 128; ntb: 64-row token blocks of this run
+  int tiles;                   // N / 128
+  int x_group_chunks;          // grouped: group g reads activation columns [g * x_group_chunks * 128, +K)
+  long long out_group_stride;  // elements between the groups' [x_rows, N] outputs
+  long long slice_stride;      // fp32 split-K slices: elements between two splits' [x_rows, N] slices
+  int cluster, silu, no_pdl;
+  const float *scale;          // [groups * N], one per stored weight row
+  const float *bias;           // [N] or null (split_k == 1 or cluster splits only)
+  __nv_bfloat16 *out_bf16;
+  float *out_f32;
+};
+
+// NSTAGE = 3: ~106 KB of shared memory, two CTAs per SM; NSTAGE = 6: ~202 KB, one CTA per SM (grids that do not
+// fill the SMs twice) - 96 KB of weight bytes in flight per SM either way
+template <int NSTAGE>
+__global__ void __launch_bounds__(NTHREADS, NSTAGE <= 3 ? 2 : 1)
+k_gemm_fp8(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, F8Params p) {
+  constexpr int SMEM_BAR = NSTAGE * F8_STAGE_BYTES;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t bar_full = base + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE;
+  const int tile = p.cluster ? blockIdx.y : blockIdx.x, split = p.cluster ? blockIdx.x : blockIdx.y;
+  const int n0 = tile * BMW;
+  const int grp = blockIdx.z / p.ntb, t0 = (blockIdx.z % p.ntb) * TOK;  // expert, first token row of this CTA
+  const int rows = p.rows - t0 < TOK ? p.rows - t0 : TOK;
+  const int c0 = split * p.chunks_per_split;
+  int c1 = c0 + p.chunks_per_split;
+  if (c1 > p.n_chunks) c1 = p.n_chunks;
+  const int nch = c1 - c0;
+
+  if (tid == 0) {
+    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncwarp();
+  if (!p.no_pdl) pdl_launch_dependents();
+  __syncthreads();
+
+  if (warp == PRODUCER_WARP) {
+    if (lane == 0) {
+      // the weight blocks are immutable: the first NSTAGE stream before griddepcontrol.wait, as in k_gemm_ws
+      const int wblk = (grp * p.tiles + tile) * p.n_chunks + c0;
+      const int xk = (grp * p.x_group_chunks + c0) * 2;  // in 64-k boxes
+      auto load_x = [&](int i, int s) {
+        const uint32_t xd = base + s * F8_STAGE_BYTES + F8_W_BYTES;
+        tma_load_2d(xd, &map_x, bar_full + 8 * s, (xk + 2 * i) * BK, t0);
+        tma_load_2d(xd + X_BYTES, &map_x, bar_full + 8 * s, (xk + 2 * i + 1) * BK, t0);
+      };
+      const int pre = nch < NSTAGE ? nch : NSTAGE;
+      for (int i = 0; i < pre; ++i) {
+        mbar_expect_tx(bar_full + 8 * i, F8_STAGE_BYTES);
+        tma_load_3d(base + i * F8_STAGE_BYTES, &map_w, bar_full + 8 * i, 0, 0, wblk + i);
+      }
+      pdl_wait();
+      for (int i = 0; i < pre; ++i) load_x(i, i);
+      for (int i = pre; i < nch; ++i) {
+        const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
+        mbar_wait(bar_empty + 8 * s, ph ^ 1);
+        mbar_expect_tx(bar_full + 8 * s, F8_STAGE_BYTES);
+        tma_load_3d(base + s * F8_STAGE_BYTES, &map_w, bar_full + 8 * s, 0, 0, wblk + i);
+        load_x(i, s);
+      }
+    }
+    __syncwarp();
+    if (p.cluster) { cluster_sync_all(); cluster_sync_all(); }
+    return;
+  }
+
+  // ---------------------------------------------------------------- consumers: warpgroup wg owns weight rows [64 wg, +64)
+  pdl_wait();
+  const int wg = warp >> 2;
+  // A fragment of m64k16 (register i of k-step j): a0 = (row r, k 2c..2c+1), a1 = (r + 8, same k), a2 = (r, k + 8),
+  // a3 = (r + 8, k + 8) with r = 16 (warp % 4) + lane / 4, c = lane % 4.  The tiled weight stores each 16-byte k group
+  // as [k0 k1 k8 k9 | k2 k3 k10 k11 | ...] (ops.tile_weight_fp8), so one 32-bit load yields a0's and a2's codes.  The
+  // 16-byte group j of row r sits at chunk j ^ (r % 8) (SWIZZLE_128B); rows r and r + 8 share that pattern.
+  const int r = wg * 64 + 16 * (warp & 3) + (lane >> 2);
+  const uint32_t roff = (uint32_t)r * F8_BK + 4 * (lane & 3);
+  const int sw = r & 7;
+  float acc[32];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+  for (int i = 0; i < nch; ++i) {
+    const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
+    mbar_wait(bar_full + 8 * s, ph);
+    const uint8_t *ws = sm + s * F8_STAGE_BYTES;
+    uint32_t a[32];
+#pragma unroll
+    for (int j = 0; j < F8_BK / 16; ++j) {
+      const uint32_t off = roff + ((uint32_t)(j ^ sw) << 4);
+      e4m3x4_to_bf16x2(*reinterpret_cast<const uint32_t *>(ws + off), a[4 * j], a[4 * j + 2]);
+      e4m3x4_to_bf16x2(*reinterpret_cast<const uint32_t *>(ws + off + 8 * F8_BK), a[4 * j + 1], a[4 * j + 3]);
+    }
+    const uint32_t xa = base + s * F8_STAGE_BYTES + F8_W_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < F8_BK / 16; ++j) wgmma_m64n64k16_ra(acc, a + 4 * j, kmajor_desc(xa + (j >> 2) * X_BYTES + (j & 3) * 32));
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_acc(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+  }
+  float *accs = reinterpret_cast<float *>(sm + ACC_OFF);
+  asm volatile("bar.sync 2, 256;" ::: "memory");
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int rr = wg * 64 + frag_row(warp, lane, h);
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<float2 *>(accs + rr * ACC_LD + frag_tok(lane, i)) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+  }
+  asm volatile("bar.sync 2, 256;" ::: "memory");
+  if (wg == 1) {
+    if (p.cluster) { cluster_sync_all(); cluster_sync_all(); }
+    return;
+  }
+
+  // epilogue (warps 0-3): thread = one weight row n, its 64 token values scaled by s[n] in fp32
+  const int q = warp;
+  const int n = n0 + q * 32 + lane;
+  float v[64];
+  {
+    const float sc = p.scale[(long long)grp * p.N + n];
+    const float4 *src = reinterpret_cast<const float4 *>(accs + (q * 32 + lane) * ACC_LD);
+#pragma unroll
+    for (int t = 0; t < 16; ++t) {
+      const float4 a = src[t];
+      v[4 * t] = a.x * sc; v[4 * t + 1] = a.y * sc; v[4 * t + 2] = a.z * sc; v[4 * t + 3] = a.w * sc;
+    }
+  }
+  if (p.cluster) {
+    // the scaled fp32 partials meet in the owner CTA of each row slice (as in k_gemm_ws), summed in split order; the
+    // bias is added once, after the sum
+    const int cs = p.cluster, RS = BMW / cs;
+    cluster_sync_all();
+    {
+      const int row = q * 32 + lane;
+      const int owner = row / RS, rl = row % RS;
+      const uint32_t dst = map_to_cta(base + (uint32_t)((split * 16) * RS + rl) * 16, owner);
+#pragma unroll
+      for (int tq = 0; tq < 16; ++tq) st_cluster_f4(dst + (uint32_t)(tq * RS) * 16, v[4 * tq], v[4 * tq + 1], v[4 * tq + 2], v[4 * tq + 3]);
+    }
+    cluster_sync_all();
+    {
+      const int e = warp * 32 + lane;
+      const int rl = e % RS, tg = e / RS;
+      const int qpt = RS / 8;
+      const int n_out = n0 + split * RS + rl;
+      const float4 *buf = reinterpret_cast<const float4 *>(sm);
+      __nv_bfloat16 *ob = p.out_bf16 + grp * p.out_group_stride + (long long)t0 * p.N;
+      const float bs = p.bias ? p.bias[n_out] : 0.f;
+      for (int tq = tg * qpt; tq < (tg + 1) * qpt; ++tq) {
+        float4 a = buf[(0 * 16 + tq) * RS + rl];
+        for (int src = 1; src < cs; ++src) {
+          const float4 b = buf[(src * 16 + tq) * RS + rl];
+          a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        }
+        const int tt = 4 * tq;
+        if (tt < rows) ob[(long long)tt * p.N + n_out] = __float2bfloat16_rn(a.x + bs);
+        if (tt + 1 < rows) ob[(long long)(tt + 1) * p.N + n_out] = __float2bfloat16_rn(a.y + bs);
+        if (tt + 2 < rows) ob[(long long)(tt + 2) * p.N + n_out] = __float2bfloat16_rn(a.z + bs);
+        if (tt + 3 < rows) ob[(long long)(tt + 3) * p.N + n_out] = __float2bfloat16_rn(a.w + bs);
+      }
+    }
+  } else if (p.silu) {
+    // SiLU(gate) * up exactly as k_gemm_ws's epilogue: rows 0-63 of the tile are gate rows, 64-127 the up rows of the
+    // same 64 columns (scales permuted alike); GEMM out -> bf16, silu -> bf16, product -> bf16
+    __nv_bfloat16 *xu = reinterpret_cast<__nv_bfloat16 *>(sm + SMEM_BAR + 256);
+    __nv_bfloat16 *xg = xu + 32 * 64;
+    const int rr = (q & 1) * 32 + lane;
+    if (q >= 2) {
+#pragma unroll
+      for (int t = 0; t < 32; ++t) xu[t * 64 + rr] = __float2bfloat16_rn(v[t]);
+    } else {
+#pragma unroll
+      for (int t = 0; t < 32; ++t) xg[t * 64 + rr] = __float2bfloat16_rn(v[32 + t]);
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    const int col = tile * 64 + rr;
+    const int inter = p.N >> 1;
+    __nv_bfloat16 *ob = p.out_bf16 + (long long)t0 * inter;
+    const int tb = q < 2 ? 0 : 32;
+#pragma unroll
+    for (int t = 0; t < 32; ++t) {
+      if (tb + t < rows) {
+        const float g = q < 2 ? __bfloat162float(__float2bfloat16_rn(v[t])) : __bfloat162float(xg[t * 64 + rr]);
+        const float u = q < 2 ? __bfloat162float(xu[t * 64 + rr]) : __bfloat162float(__float2bfloat16_rn(v[32 + t]));
+        const float sg = __bfloat162float(__float2bfloat16_rn(g / (1.f + expf(-g))));
+        ob[(long long)(tb + t) * inter + col] = __float2bfloat16_rn(sg * u);
+      }
+    }
+  } else if (p.n_split == 1) {
+    const float bs = p.bias ? p.bias[n] : 0.f;
+    __nv_bfloat16 *ob = p.out_bf16 + grp * p.out_group_stride + (long long)t0 * p.N;
+#pragma unroll
+    for (int t = 0; t < TOK; ++t)
+      if (t < rows) ob[(long long)t * p.N + n] = __float2bfloat16_rn(v[t] + bs);
+  } else {
+    float *o = p.out_f32 + split * p.slice_stride + (long long)t0 * p.N;
+#pragma unroll
+    for (int t = 0; t < TOK; ++t)
+      if (t < rows) o[(long long)t * p.N + n] = v[t];
+  }
+}
+
 }  // namespace gemm
 }  // namespace pia
 
@@ -482,6 +732,9 @@ struct pia_gemm_plan {
   // stream-K mode
   int stream_k, sk_grid;
   SkParams sk;
+  // fp8 weight mode (pia_gemm_plan_create_fp8 / _grouped_fp8): k_gemm_fp8 with `f`, up to x_rows rows per run
+  int fp8, groups, x_rows;
+  F8Params f;
 };
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -615,8 +868,17 @@ extern "C" int pia_gemm_plan_set_pdl(pia_gemm_plan_t *g, int on) {
   g->no_pdl = on ? 0 : 1;
   return PIA_OK;
 }
-extern "C" int pia_gemm_plan_splits(const pia_gemm_plan_t *g) { return g ? (g->p.cluster ? 1 : g->p.n_split) : 0; }
+extern "C" int pia_gemm_plan_splits(const pia_gemm_plan_t *g) {
+  if (g && g->fp8) return g->f.cluster ? 1 : g->f.n_split;
+  return g ? (g->p.cluster ? 1 : g->p.n_split) : 0;
+}
 extern "C" int pia_gemm_plan_set_silu(pia_gemm_plan_t *g, int on) {
+  if (g && g->fp8) {
+    PIA_REQUIRE(g->f.n_split == 1 && !g->f.bias && g->groups == 1,
+                "the SiLU*up epilogue needs split_k == 1, no bias and one group");
+    g->f.silu = on ? 1 : 0;
+    return PIA_OK;
+  }
   PIA_REQUIRE(g && g->p.n_split == 1 && !g->stream_k && g->p.N % BMW == 0, "the SiLU*up epilogue needs split_k == 1 and N %% 128 == 0");
   g->p.silu = on ? 1 : 0;
   return PIA_OK;
@@ -654,10 +916,98 @@ extern "C" int pia_gemm_plan_create_grouped(const void *d_w, int groups, int N, 
   return PIA_OK;
 }
 
+// fp8 weights, tiled by ops.tile_weight_fp8: [groups][N/128][K/128] contiguous 16 KB blocks of 128 rows x 128 e4m3
+// bytes, one SWIZZLE_128B TMA box each
+static int encode_tiled_w_fp8(CUtensorMap *m, const void *base, uint64_t n_blocks) {
+  EncodeTiledFn fn = get_encode();
+  PIA_REQUIRE(fn, "cuTensorMapEncodeTiled not available in this driver");
+  cuuint64_t dims[3] = {(cuuint64_t)F8_BK, (cuuint64_t)BMW, n_blocks};
+  cuuint64_t strides[2] = {(cuuint64_t)F8_BK, (cuuint64_t)F8_BK * BMW};
+  cuuint32_t box[3] = {F8_BK, BMW, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void *>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return PIA_ERR_CUDA; }
+  return PIA_OK;
+}
+
+static int f8_plan_create(const void *d_w, const void *d_scale, const void *d_bias, int groups, int N, int K,
+                          const void *d_x, int x_rows, int split_k, pia_gemm_plan_t **out) {
+  PIA_REQUIRE(d_w && d_scale && d_x && out, "null argument");
+  PIA_REQUIRE(groups >= 1 && groups <= 4096 && N > 0 && N % BMW == 0 && K > 0 && K % F8_BK == 0,
+              "the fp8 GEMM needs N %% %d == 0 and K %% %d == 0", BMW, F8_BK);
+  PIA_REQUIRE(x_rows >= TOK, "the activation buffer must hold at least %d rows", TOK);
+  PIA_REQUIRE((reinterpret_cast<uintptr_t>(d_w) & 15) == 0 && (reinterpret_cast<uintptr_t>(d_x) & 15) == 0, "operands must be 16-byte aligned");
+  const int n_chunks = K / F8_BK;
+  const int want_cluster = (split_k == -2 || split_k == -4 || split_k == -8) ? -split_k : 0;
+  PIA_REQUIRE(split_k >= 1 || want_cluster, "fp8 plans take split_k >= 1 or a cluster split of 2, 4 or 8 CTAs");
+  PIA_REQUIRE(groups == 1 || split_k == 1, "a grouped fp8 plan has one K split");
+  if (want_cluster) split_k = want_cluster;
+  if (split_k > n_chunks) split_k = n_chunks;
+  pia_gemm_plan *g = new (std::nothrow) pia_gemm_plan();
+  PIA_REQUIRE(g, "out of host memory");
+  F8Params &f = g->f;
+  f.N = N; f.n_chunks = n_chunks; f.tiles = N / BMW;
+  f.chunks_per_split = (n_chunks + split_k - 1) / split_k;
+  f.n_split = (n_chunks + f.chunks_per_split - 1) / f.chunks_per_split;
+  f.rows = TOK; f.ntb = 1;
+  f.x_group_chunks = groups > 1 ? n_chunks : 0;
+  f.out_group_stride = (long long)x_rows * N;
+  f.slice_stride = (long long)x_rows * N;
+  f.cluster = 0; f.silu = 0; f.no_pdl = 0;
+  f.scale = (const float *)d_scale; f.bias = (const float *)d_bias;
+  f.out_bf16 = nullptr; f.out_f32 = nullptr;
+  if (want_cluster && f.n_split != want_cluster) { delete g; set_error("K = %d is too short for %d cluster splits", K, want_cluster); return PIA_ERR_INVALID; }
+  f.cluster = want_cluster;
+  if (d_bias && f.n_split > 1 && !f.cluster) { delete g; set_error("a bias needs split_k == 1 or a cluster split"); return PIA_ERR_INVALID; }
+  g->fp8 = 1; g->groups = groups; g->x_rows = x_rows;
+  int rc = encode_tiled_w_fp8(&g->map_w, d_w, (uint64_t)groups * f.tiles * n_chunks);
+  if (rc == PIA_OK) rc = encode_2d(&g->map_x, d_x, (uint64_t)groups * K, (uint64_t)x_rows, BK, TOK, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc == PIA_OK) {
+    int n_sm = 132, dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    g->nstage = f.tiles * f.n_split * groups <= n_sm ? 6 : 3;
+    cudaError_t e = cudaFuncSetAttribute(k_gemm_fp8<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, f8_smem_total(3));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_fp8<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, f8_smem_total(6));
+    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); rc = PIA_ERR_CUDA; }
+  }
+  if (rc != PIA_OK) { delete g; return rc; }
+  *out = g;
+  return PIA_OK;
+}
+
+extern "C" int pia_gemm_plan_create_fp8(const void *d_w, const void *d_scale, const void *d_bias, int N, int K,
+                                        const void *d_x, int x_rows, int split_k, pia_gemm_plan_t **out) {
+  return f8_plan_create(d_w, d_scale, d_bias, 1, N, K, d_x, x_rows, split_k, out);
+}
+
+extern "C" int pia_gemm_plan_create_grouped_fp8(const void *d_w, const void *d_scale, int groups, int N, int K,
+                                                const void *d_x, int x_rows, pia_gemm_plan_t **out) {
+  return f8_plan_create(d_w, d_scale, nullptr, groups, N, K, d_x, x_rows, 1, out);
+}
+
 struct PdlScope { int on; explicit PdlScope(int off) : on(off) { if (on) ++pia::g_pdl_off; } ~PdlScope() { if (on) --pia::g_pdl_off; } };
+
+static int f8_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream) {
+  PIA_REQUIRE(rows >= 1 && rows <= g->x_rows, "rows %d outside [1,%d]", rows, g->x_rows);
+  PdlScope pdl_scope(g->no_pdl);
+  F8Params f = g->f;
+  f.rows = rows; f.ntb = (rows + TOK - 1) / TOK; f.no_pdl = g->no_pdl;
+  if (f.n_split == 1 || f.cluster) f.out_bf16 = (__nv_bfloat16 *)d_out; else f.out_f32 = (float *)d_out;
+  const unsigned z = (unsigned)(g->groups * f.ntb);
+  const dim3 grid = f.cluster ? dim3(f.n_split, f.tiles, z) : dim3(f.tiles, f.n_split, z);
+  const unsigned cs = f.cluster ? (unsigned)f.cluster : 1u;
+  if (g->nstage == 6) PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_fp8<6>, grid, dim3(NTHREADS), f8_smem_total(6), (cudaStream_t)stream, cs, g->map_w, g->map_x, f));
+  else PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_fp8<3>, grid, dim3(NTHREADS), f8_smem_total(3), (cudaStream_t)stream, cs, g->map_w, g->map_x, f));
+  count_launch();
+  return PIA_OK;
+}
 
 extern "C" int pia_gemm_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream) {
   PIA_REQUIRE(g && d_out, "null argument");
+  if (g->fp8) return f8_run(g, rows, d_out, stream);
   PIA_REQUIRE(rows >= 1 && rows <= TOK, "rows %d outside [1,%d]", rows, TOK);
   PdlScope pdl_scope(g->no_pdl);
   if (g->stream_k) {

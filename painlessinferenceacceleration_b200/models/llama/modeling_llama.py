@@ -48,6 +48,69 @@ class LlamaMLP(nn.Module):
         self.down_proj = nn.Linear(cfg.intermediate_size, cfg.hidden_size, **kw)
 
 
+def _gate_up_order(w, inverse=False, vec=False):
+    """[..., gate (I rows); up (I rows), K] <-> the SiLU*up epilogue's row order (ops.interleave_gate_up), for any
+    leading dims (stacked experts); vec: per-row values [..., 2I] (the scales)"""
+    x = w.unsqueeze(-1) if vec else w
+    two_i, K = x.shape[-2:]
+    lead = x.shape[:-2]
+    if inverse:
+        y = x.reshape(*lead, two_i // 128, 2, 64, K).transpose(-4, -3)
+    else:
+        y = x.reshape(*lead, 2, two_i // 128, 64, K).transpose(-4, -3)
+    y = y.reshape(*lead, two_i, K).contiguous()
+    return y.squeeze(-1) if vec else y
+
+
+class Fp8Linear(nn.Module):
+    """fp8 (e4m3) weight of one projection, or of G stacked ones (the MoE experts), stored once, in the fp8 GEMM's
+    HBM-tiled layout: `qweight` uint8 (ops.tile_weight_fp8), `scale` fp32, one per stored row (ops.quantize_fp8).
+    `interleaved`: a fused gate/up weight whose rows are stored in the SiLU*up epilogue's order."""
+
+    def __init__(self, w, interleaved=False):
+        super().__init__()
+        self.shape = tuple(w.shape)
+        self.interleaved = interleaved
+        if interleaved:   # quantisation is per row, so reordering rows first gives the same codes and scales
+            w = _gate_up_order(w)
+        q, s = ops.quantize_fp8(w)
+        self.qweight = nn.Parameter(ops.tile_weight_fp8(q), requires_grad=False)
+        self.scale = nn.Parameter(s, requires_grad=False)
+
+    def codes(self):
+        """(q e4m3 [..., N, K], s fp32 [..., N]) in the checkpoint's row order"""
+        q, s = ops.untile_weight_fp8(self.qweight), self.scale.data
+        if self.interleaved:
+            q = _gate_up_order(q.view(torch.uint8), inverse=True).view(torch.float8_e4m3fn)
+            s = _gate_up_order(s, inverse=True, vec=True)
+        return q, s
+
+    def dequantize(self):
+        """the weight the fp8 GEMM multiplies with: float(q) * s, fp32"""
+        q, s = self.codes()
+        return q.float() * s.unsqueeze(-1)
+
+
+class Fp8Rows(nn.Module):
+    """rows [r0, r1) of a fused Fp8Linear under their HF name (q_proj / k_proj / v_proj, gate_proj / up_proj); the
+    bytes belong to the fused weight, `bias` (Qwen2) stays the bf16 parameter it was"""
+
+    def __init__(self, fused, r0, r1, bias=None):
+        super().__init__()
+        self._fused = (fused,)   # a tuple: not a submodule, its parameters are counted once
+        self.r0, self.r1 = r0, r1
+        self.shape = (r1 - r0, fused.shape[-1])
+        self.bias = bias
+
+    def codes(self):
+        q, s = self._fused[0].codes()
+        return q[self.r0:self.r1], s[self.r0:self.r1]
+
+    def dequantize(self):
+        q, s = self.codes()
+        return q.float() * s.unsqueeze(-1)
+
+
 class LlamaDecoderLayer(nn.Module):
     qkv_bias = False   # biases on q/k/v (Qwen2); o_proj never has one
 
@@ -83,6 +146,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         self.model = self.model_cls(config, device, dtype)
         self.lm_head = nn.Linear(config.hidden_size, config.vocab_size, bias=False, device=device, dtype=dtype)
         self._fused = False
+        self._fp8 = False
         for p_ in self.parameters():  # inference only: no autograd state on the hot path
             p_.requires_grad_(False)
 
@@ -99,20 +163,29 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                 p.normal_(0.0, std, generator=gen)
         return self
 
-    @classmethod
-    def from_pretrained(cls, path, torch_dtype=torch.bfloat16, device=None, **kwargs):
-        """HF checkpoint directory (config.json + *.safetensors / pytorch_model*.bin) -> model on the GPU"""
-        from transformers import AutoConfig
-        config = AutoConfig.from_pretrained(path)
-        model = cls(config, device=device, dtype=torch_dtype)
+    @staticmethod
+    def _shards(path):
         files = sorted(glob.glob(os.path.join(path, '*.safetensors')))
-        own = dict(model.named_parameters())
-        seen = set()
         if files:
             from safetensors.torch import load_file
-            shards = (load_file(f) for f in files)
-        else:
-            shards = (torch.load(f, map_location='cpu') for f in sorted(glob.glob(os.path.join(path, 'pytorch_model*.bin'))))
+            return (load_file(f) for f in files)
+        return (torch.load(f, map_location='cpu') for f in sorted(glob.glob(os.path.join(path, 'pytorch_model*.bin'))))
+
+    @classmethod
+    def from_pretrained(cls, path, torch_dtype=torch.bfloat16, device=None, quantization=None, **kwargs):
+        """HF checkpoint directory (config.json + *.safetensors / pytorch_model*.bin) -> model on the GPU.
+        quantization='fp8': the decoder projections become fp8 weights as they arrive (see quantize_fp8); the bf16
+        decoder never exists on the GPU."""
+        from transformers import AutoConfig
+        if quantization not in (None, 'fp8'):
+            raise ValueError(f'quantization={quantization!r}: only None and \'fp8\' are supported')
+        config = AutoConfig.from_pretrained(path)
+        if quantization == 'fp8':
+            return cls._from_pretrained_fp8(path, config, device)
+        model = cls(config, device=device, dtype=torch_dtype)
+        own = dict(model.named_parameters())
+        seen = set()
+        shards = cls._shards(path)
         with torch.no_grad():
             for sd in shards:
                 for k, v in model._convert_checkpoint_keys(sd).items():
@@ -128,6 +201,90 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             raise RuntimeError(f'checkpoint is missing {len(missing)} tensors, e.g. {missing[:4]}')
         return model
 
+    # the parameters of a decoder layer that fp8 mode quantises (relative to the layer)
+    _fp8_params = ('self_attn.q_proj.weight', 'self_attn.k_proj.weight', 'self_attn.v_proj.weight',
+                   'self_attn.o_proj.weight', 'mlp.gate_proj.weight', 'mlp.up_proj.weight', 'mlp.down_proj.weight')
+
+    @classmethod
+    def _fp8_skeleton(cls, config, device):
+        """the model on the meta device with everything but the quantised projections allocated (uninitialised) on
+        the GPU.  Returns (model, {name: allocated parameter}, layer_of(name) -> layer index of a quantised projection
+        or None, materialise(name) -> that projection allocated in bf16 on the GPU)"""
+        dev = device if device is not None else torch.device('cuda', torch.cuda.current_device())
+        model = cls(config, device='meta')
+
+        def layer_of(name):
+            parts = name.split('.')
+            if name.startswith('model.layers.') and '.'.join(parts[3:]) in cls._fp8_params:
+                return int(parts[2])
+            return None
+
+        def materialise(name):
+            mod_name, _, pname = name.rpartition('.')
+            mod = model.get_submodule(mod_name)
+            old = getattr(mod, pname)
+            setattr(mod, pname, nn.Parameter(torch.empty(old.shape, dtype=old.dtype, device=dev), requires_grad=False))
+            return getattr(mod, pname)
+
+        own = {name: materialise(name) for name, _ in list(model.named_parameters()) if layer_of(name) is None}
+        return model, own, layer_of, materialise
+
+    @classmethod
+    @torch.no_grad()
+    def build_fp8(cls, config, fill_rest, fill_weight, device=None):
+        """An fp8 model without a checkpoint and without its bf16 decoder ever existing: fill_rest(model) initialises
+        the parameters that stay bf16 (the quantised projections are still meta tensors then, and may be skipped);
+        then, one layer at a time, fill_weight(name, tensor) fills each projection in a bf16 buffer (HF names, e.g.
+        'model.layers.3.self_attn.q_proj.weight'), which is fused, quantised and freed.  Gives the bytes of
+        quantize_fp8() on a bf16 model filled the same way."""
+        model, _, _, materialise = cls._fp8_skeleton(config, device)
+        fill_rest(model)
+        for li, layer in enumerate(model.model.layers):
+            for p in cls._fp8_params:
+                name = f'model.layers.{li}.{p}'
+                fill_weight(name, materialise(name))
+            model._fuse_layer(layer)
+            model._quantize_layer(layer)
+        model._fused = True
+        model._fp8 = True
+        return model
+
+    @classmethod
+    @torch.no_grad()
+    def _from_pretrained_fp8(cls, path, config, device):
+        """The model is built on the meta device; everything but the quantised projections is allocated on the GPU up
+        front.  A layer's projections wait on the host until the layer is complete, then that one layer is allocated
+        in bf16, filled, fused and quantised, so the GPU holds the fp8 model plus at most one bf16 layer."""
+        model, own, layer_of, materialise = cls._fp8_skeleton(config, device)
+        n_layers = len(model.model.layers)
+        pending = {li: {} for li in range(n_layers)}
+        seen = set()
+        for sd in cls._shards(path):
+            for k, v in model._convert_checkpoint_keys(sd).items():
+                li = layer_of(k)
+                if li is not None and li in pending:
+                    pending[li][k] = v
+                    if len(pending[li]) == len(cls._fp8_params):
+                        for name, t in pending.pop(li).items():
+                            materialise(name).copy_(t.to(torch.bfloat16))
+                        layer = model.model.layers[li]
+                        model._fuse_layer(layer)
+                        model._quantize_layer(layer)
+                elif k in own:
+                    own[k].copy_(v.to(torch.bfloat16))
+                    seen.add(k)
+        if 'lm_head.weight' not in seen and getattr(config, 'tie_word_embeddings', False):
+            model.lm_head.weight.copy_(model.model.embed_tokens.weight)
+            seen.add('lm_head.weight')
+        missing = [k for k in own if k not in seen]
+        missing += [f'model.layers.{li}.{p}' for li, got in pending.items() for p in cls._fp8_params
+                    if f'model.layers.{li}.{p}' not in got]
+        if missing:
+            raise RuntimeError(f'checkpoint is missing {len(missing)} tensors, e.g. {missing[:4]}')
+        model._fused = True
+        model._fp8 = True
+        return model
+
     def _convert_checkpoint_keys(self, sd):
         """checkpoint tensor names -> this module tree's names (identity for Llama / Mistral)"""
         return sd
@@ -138,18 +295,21 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         if self._fused:
             return
         for layer in self.model.layers:
-            a = layer.self_attn
-            w = torch.cat([a.q_proj.weight.data, a.k_proj.weight.data, a.v_proj.weight.data], dim=0).contiguous()
-            nq, nk = a.q_proj.weight.shape[0], a.k_proj.weight.shape[0]
-            a.q_proj.weight.data, a.k_proj.weight.data, a.v_proj.weight.data = w[:nq], w[nq:nq + nk], w[nq + nk:]
-            a.qkv_weight = w
-            a.qkv_bias = None
-            if a.q_proj.bias is not None:
-                bias = torch.cat([a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data]).contiguous()
-                a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data = bias[:nq], bias[nq:nq + nk], bias[nq + nk:]
-                a.qkv_bias = bias
-            self._fuse_mlp(layer)
+            self._fuse_layer(layer)
         self._fused = True
+
+    def _fuse_layer(self, layer):
+        a = layer.self_attn
+        w = torch.cat([a.q_proj.weight.data, a.k_proj.weight.data, a.v_proj.weight.data], dim=0).contiguous()
+        nq, nk = a.q_proj.weight.shape[0], a.k_proj.weight.shape[0]
+        a.q_proj.weight.data, a.k_proj.weight.data, a.v_proj.weight.data = w[:nq], w[nq:nq + nk], w[nq + nk:]
+        a.qkv_weight = w
+        a.qkv_bias = None
+        if a.q_proj.bias is not None:
+            bias = torch.cat([a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data]).contiguous()
+            a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data = bias[:nq], bias[nq:nq + nk], bias[nq + nk:]
+            a.qkv_bias = bias
+        self._fuse_mlp(layer)
 
     def _fuse_mlp(self, layer):
         m = layer.mlp
@@ -157,6 +317,105 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         ni = m.gate_proj.weight.shape[0]
         m.gate_proj.weight.data, m.up_proj.weight.data = w[:ni], w[ni:]
         m.gate_up_weight = w
+
+    # ------------------------------------------------------------------ fp8 (e4m3) weight-only mode
+    def _fp8_weight_shapes(self, layer):
+        """(name, shape) of every weight of a fused layer that fp8 mode quantises"""
+        a, m = layer.self_attn, layer.mlp
+        return [('qkv', a.qkv_weight.shape), ('o_proj', a.o_proj.weight.shape), ('gate_up', m.gate_up_weight.shape),
+                ('down_proj', m.down_proj.weight.shape)]
+
+    @torch.no_grad()
+    def quantize_fp8(self):
+        """Convert the decoder projections (fused q/k/v, o, fused gate/up, down; Mixtral's experts) to per-row e4m3
+        weights with fp32 scales (ops.quantize_fp8), in place and one layer at a time: each bf16 weight is freed once
+        its fp8 copy exists.  Embeddings, lm_head, norms, the router and QKV biases stay bf16.  Every weight must have
+        both dimensions divisible by 128; otherwise ValueError before anything is converted."""
+        if self._fp8:
+            return self
+        self.fuse()
+        for li, layer in enumerate(self.model.layers):
+            for name, shape in self._fp8_weight_shapes(layer):
+                if shape[-1] % 128 or shape[-2] % 128:
+                    raise ValueError(f'layer {li} {name} {tuple(shape)}: fp8 weights need both dimensions divisible by 128')
+        self._rt = None                               # drops the bf16 GEMM plans and the buffers bound to them
+        self.__dict__.pop('_tiled_weights', None)     # and the bf16 HBM-tiled copies
+        for layer in self.model.layers:
+            self._quantize_layer(layer)
+        self._fp8 = True
+        return self
+
+    def _quantize_layer(self, layer):
+        a = layer.self_attn
+        nq, nk = a.q_proj.weight.shape[0], a.k_proj.weight.shape[0]
+        qkv = Fp8Linear(a.qkv_weight)
+        a.qkv_fp8 = qkv
+        a.q_proj = Fp8Rows(qkv, 0, nq, a.q_proj.bias)
+        a.k_proj = Fp8Rows(qkv, nq, nq + nk, a.k_proj.bias)
+        a.v_proj = Fp8Rows(qkv, nq + nk, qkv.shape[0], a.v_proj.bias)
+        a.qkv_weight = None
+        a.o_proj = Fp8Linear(a.o_proj.weight.data)
+        self._quantize_mlp(layer)
+
+    def _quantize_mlp(self, layer):
+        m = layer.mlp
+        ni = m.gate_proj.weight.shape[0]
+        gu = Fp8Linear(m.gate_up_weight, interleaved=True)
+        m.gate_up_fp8 = gu
+        m.gate_proj, m.up_proj = Fp8Rows(gu, 0, ni), Fp8Rows(gu, ni, 2 * ni)
+        m.gate_up_weight = None
+        m.down_proj = Fp8Linear(m.down_proj.weight.data)
+
+    @staticmethod
+    def _fp8_split(w, n_sm):
+        """K splits of an fp8 plan: 1 when the 128-row tiles alone come close to filling the SMs (or the plan uses the
+        SiLU epilogue), else the smallest 2 / 4 / 8-CTA cluster split that does (cluster splits add the bias once and
+        write bf16)"""
+        tiles, chunks = w.shape[-2] // 128, w.shape[-1] // 128
+        want = (n_sm * 7) // 8
+        if tiles >= want:
+            return 1
+        best = 1
+        for s in (2, 4, 8):
+            if chunks >= s and -(-chunks // -(-chunks // s)) == s:
+                best = s
+                if tiles * s >= want:
+                    break
+        return -best if best > 1 else 1
+
+    def _fp8_plans(self, b):
+        """fp8 GEMM plans of one activation buffer set (the decode rows or the prefill pass's 256), on the buffers;
+        there is no other path for fp8 weights, so the bf16 GEMM selection knobs are refused"""
+        plans = getattr(b, 'fp8_plans', None)
+        if plans is not None:
+            return plans
+        if os.environ.get('PIA_GEMM', '1') == '0' or 'PIA_GEMM_SET' in os.environ:
+            raise ValueError('this model holds fp8 weights, which only the fp8 GEMM runs: PIA_GEMM=0 / PIA_GEMM_SET '
+                             'do not apply')
+        hid = self.config.hidden_size
+        b.fp8_out = torch.zeros((b.rows, hid), dtype=torch.bfloat16, device=b.y.device)
+        n_sm = torch.cuda.get_device_properties(b.y.device).multi_processor_count
+        plans = {'layers': [self._layer_fp8_plans(layer, b, n_sm) for layer in self.model.layers]}
+        b.fp8_plans = plans
+        return plans
+
+    def _attn_fp8_plans(self, layer, b, n_sm):
+        a = layer.self_attn
+        qkv, o = a.qkv_fp8, a.o_proj
+        bias = a.qkv_bias.float() if a.qkv_bias is not None else None
+        return {'qkv': ops.Gemm.fp8(qkv.qweight, qkv.scale, b.y, bias=bias, split_k=self._fp8_split(qkv, n_sm),
+                                    out=b.qkv),
+                'o': ops.Gemm.fp8(o.qweight, o.scale, b.attn, split_k=self._fp8_split(o, n_sm), out=b.fp8_out)}
+
+    def _layer_fp8_plans(self, layer, b, n_sm):
+        m = layer.mlp
+        plans = self._attn_fp8_plans(layer, b, n_sm)
+        if getattr(b, 'act', None) is None or b.act.shape[0] != b.rows:
+            b.act = torch.zeros((b.rows, self.config.intermediate_size), dtype=torch.bfloat16, device=b.y.device)
+        plans['gate_up_silu'] = ops.Gemm.fp8(m.gate_up_fp8.qweight, m.gate_up_fp8.scale, b.y, out=b.act).set_silu()
+        plans['down'] = ops.Gemm.fp8(m.down_proj.qweight, m.down_proj.scale, b.act,
+                                     split_k=self._fp8_split(m.down_proj, n_sm), out=b.fp8_out)
+        return plans
 
     # ------------------------------------------------------------------ geometry / tables
     def geometry(self):
@@ -199,6 +458,11 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         plans = getattr(rt, 'gemm_plans', None)
         if plans is not None:
             return plans
+        if self._fp8:   # fp8 weights: the fp8 plans of both buffer sets instead, built here, outside any capture
+            self._fp8_plans(rt.decode_bufs)
+            self._fp8_plans(rt.prefill_bufs)
+            rt.gemm_plans = False
+            return False
         import os
         if os.environ.get('PIA_GEMM', '1') == '0' or rt.max_nodes != 64:
             rt.gemm_plans = False
@@ -299,13 +563,15 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         pf['dirty'] = True
 
     # ------------------------------------------------------------------ the verify forward on static buffers
-    def _mlp(self, rt, layer, y, plans=None, pf=None):
-        """returns (x, parts): the MLP output as a bf16 tensor or as fp32 split-K slices for the next rmsnorm"""
+    def _mlp(self, rt, layer, y, plans=None, pf=None, b=None):
+        """returns (x, parts): the MLP output as a bf16 tensor or as fp32 split-K slices for the next rmsnorm.
+        b: the buffer set y belongs to (default: the decode buffers)"""
         m = layer.mlp
         if plans:
-            b = rt.decode_bufs
+            b = b if b is not None else rt.decode_bufs
+            rows = y.shape[0]   # 64 for the bf16 plans; every buffer row for the fp8 plans
             if 'gate_up_silu' in plans:
-                plans['gate_up_silu'].run(64, out=b.act)
+                plans['gate_up_silu'].run(rows, out=b.act)
             else:
                 if 'gate_up' in plans:
                     plans['gate_up'].run(64, out=b.gu)
@@ -315,7 +581,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                     self._prefetch(pf, [(m.down_proj.weight, pf['down'], 0)])
                 ops.silu_mul(b.gu, b.act)
             if 'down' in plans:
-                o = plans['down'].run(64)
+                o = plans['down'].run(rows)
                 return (o, None) if plans['down'].splits == 1 else (None, o)
             return torch.mm(b.act, m.down_proj.weight.t()), None
         gu = torch.mm(y, m.gate_up_weight.t())
@@ -334,8 +600,11 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         g = rt.g
         eps = self.config.rms_norm_eps
         ops.embed_gather(self.model.embed_tokens.weight, b.ids, b.n_total, b.h)
-        plans = self._gemm_plans(rt) if b is rt.decode_bufs else False
-        pf = self._prefetch_cfg(rt) if plans else False
+        if self._fp8:   # every projection of every buffer set on the fp8 plans, over all rows of the buffers
+            plans, rows = self._fp8_plans(b), b.rows
+        else:
+            plans, rows = (self._gemm_plans(rt) if b is rt.decode_bufs else False), 64
+        pf = self._prefetch_cfg(rt) if plans and not self._fp8 else False
         fused_attn = b is rt.decode_bufs and os.environ.get('PIA_ATTN_FUSED', '0') != '0' and \
             (b.slots.batch == 1 or b.slots.kv_slot_stride != 0)
         x, parts, resid_in = b.h, None, None  # norm(x | parts, resid_in) -> (resid = x + resid_in, y = norm(resid))
@@ -351,7 +620,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             norm(layer.input_layernorm.weight)
             a = layer.self_attn
             if lp and 'qkv' in lp:
-                lp['qkv'].run(64, out=b.qkv)
+                lp['qkv'].run(rows, out=b.qkv)
             elif a.qkv_bias is not None:   # bias added in fp32 before the one bf16 rounding, as F.linear does
                 torch.addmm(a.qkv_bias, b.y, a.qkv_weight.t(), out=b.qkv)
             else:
@@ -368,19 +637,19 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                                    rt.rope_sin, b.q, rt.k_layer(li, b.kv_slot), rt.v_layer(li, b.kv_slot), rt.max_seq)
                 rt.plan.forward(li, b.q, b.mask, b.slots, b.attn)
             if lp and 'o' in lp:
-                o = lp['o'].run(64)
+                o = lp['o'].run(rows)
                 x, parts, resid_in = (o, None, b.resid) if lp['o'].splits == 1 else (None, o, b.resid)
             else:
                 x, parts, resid_in = torch.mm(b.attn, a.o_proj.weight.t()), None, b.resid
             norm(layer.post_attention_layernorm.weight)
-            x, parts = self._mlp(rt, layer, b.y, lp, pf)
+            x, parts = self._mlp(rt, layer, b.y, lp, pf, b=b)
         if pf and pf.pop('dirty', False):  # join the side stream (required before a capture ends)
             torch.cuda.current_stream().wait_stream(pf['side'])
         if last_only:
             return
         norm(self.model.norm.weight)
         if b.logits is not None:
-            if plans:
+            if plans and 'lm_head' in plans:
                 plans['lm_head'].run(64, out=b.logits)
             else:
                 torch.mm(b.y, self.lm_head.weight.t(), out=b.logits)

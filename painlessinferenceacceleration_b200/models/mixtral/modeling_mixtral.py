@@ -13,7 +13,7 @@ import torch
 from torch import nn
 
 from ...common import ops
-from ..llama.modeling_llama import LlamaDecoderLayer, LlamaForCausalLM, LlamaModel
+from ..llama.modeling_llama import Fp8Linear, LlamaDecoderLayer, LlamaForCausalLM, LlamaModel
 from ..mistral.modeling_mistral import warn_sliding_window
 
 
@@ -111,13 +111,55 @@ class MixtralForCausalLM(LlamaForCausalLM):
         return {'moe_gate_up': ops.Gemm(moe.experts.gate_up_proj.data.view(E * two_i, H), b.y),
                 'moe_down': ops.Gemm.grouped(moe.experts.down_proj.data, b.moe_act)}
 
-    def _mlp(self, rt, layer, y, plans=None, pf=None):
+    # ------------------------------------------------------------------ fp8: the experts as stacked fp8 weights
+    # the experts' stacks are quantised once _convert_checkpoint_keys has assembled them
+    _fp8_params = ('self_attn.q_proj.weight', 'self_attn.k_proj.weight', 'self_attn.v_proj.weight',
+                   'self_attn.o_proj.weight', 'mlp.experts.gate_up_proj', 'mlp.experts.down_proj')
+
+    def _fp8_weight_shapes(self, layer):
+        a, ex = layer.self_attn, layer.mlp.experts
+        return [('qkv', a.qkv_weight.shape), ('o_proj', a.o_proj.weight.shape),
+                ('experts.gate_up_proj', ex.gate_up_proj.shape), ('experts.down_proj', ex.down_proj.shape)]
+
+    def _quantize_mlp(self, layer):
+        ex = layer.mlp.experts
+        gu = Fp8Linear(ex.gate_up_proj.data, interleaved=True)   # per expert: 64 gate + 64 up rows per tile
+        del ex.gate_up_proj
+        ex.gate_up_proj = gu
+        dn = Fp8Linear(ex.down_proj.data)
+        del ex.down_proj
+        ex.down_proj = dn
+
+    def _layer_fp8_plans(self, layer, b, n_sm):
+        """qkv / o as in Llama; all experts' gate_up as ONE fp8 launch with the SiLU*up epilogue over the stacked
+        [E * 2I, H] weight (writes act [rows, E * I]), all experts' down projections as one grouped fp8 launch"""
+        plans = self._attn_fp8_plans(layer, b, n_sm)
+        ex = layer.mlp.experts
+        E, two_i, H = ex.gate_up_proj.shape
+        dev = b.y.device
+        if getattr(b, 'moe_act', None) is None or b.moe_act.shape[0] != b.rows:
+            b.moe_act = torch.zeros((b.rows, E * (two_i // 2)), dtype=torch.bfloat16, device=dev)
+            b.moe_out = torch.zeros((b.rows, H), dtype=torch.bfloat16, device=dev)
+            b.moe_dense = torch.zeros((b.rows, E), dtype=torch.bfloat16, device=dev)
+        gq = ex.gate_up_proj.qweight
+        plans['moe_gate_up_silu'] = ops.Gemm.fp8(gq.view(-1, *gq.shape[2:]), ex.gate_up_proj.scale.view(-1), b.y,
+                                                 out=b.moe_act).set_silu()
+        plans['moe_down'] = ops.Gemm.grouped_fp8(ex.down_proj.qweight, ex.down_proj.scale, b.moe_act)
+        return plans
+
+    def _mlp(self, rt, layer, y, plans=None, pf=None, b=None):
         moe = layer.mlp
         if plans:
-            b = rt.decode_bufs
+            b = b if b is not None else rt.decode_bufs
             E = moe.num_experts
             inter = moe.experts.down_proj.shape[2]
             ops.moe_router(y, moe.gate.weight, moe.top_k, b.moe_dense)              # :721-727 in one kernel
+            if 'moe_gate_up_silu' in plans:                                         # fp8: all rows of the buffers
+                rows = y.shape[0]
+                plans['moe_gate_up_silu'].run(rows, out=b.moe_act)
+                ye = plans['moe_down'].run(rows)                                    # [E, rows, H]
+                ops.moe_combine(ye, b.moe_dense, b.moe_out)
+                return b.moe_out, None
             plans['moe_gate_up'].run(64, out=b.moe_gu)
             ops.silu_mul(b.moe_gu.view(b.rows * E, 2 * inter), b.moe_act.view(b.rows * E, inter))
             ye = plans['moe_down'].run(64)                                          # [E, 64, H]
