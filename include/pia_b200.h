@@ -185,7 +185,7 @@ typedef struct {
 typedef struct pia_attn_plan pia_attn_plan_t;
 
 typedef struct {
-  int32_t n_q_heads, n_kv_heads, head_dim; /* head_dim 128 or 64                                     */
+  int32_t n_q_heads, n_kv_heads, head_dim; /* head_dim 128 or 64 (others: PIA_ERR_UNSUPPORTED)        */
   int32_t max_seq;                         /* rows of the KV cache (max_length + decoding_length + 1) */
   int32_t max_nodes;                       /* 64 (W=1) or 128 (W=2)                                  */
   int32_t n_layers;

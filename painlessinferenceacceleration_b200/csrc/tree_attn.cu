@@ -12,11 +12,13 @@
 // Warp roles (288 threads):  warps 0-7 = two consumer warpgroups, each owning 64 rows (wgmma M = 64): they stage Q
 //                            (and, fused, the draft tile), issue the MMAs and run the softmax in registers,
 //                            warp 8 = TMA producer (K/V tiles of 128 keys, 2-stage ring, V on its own barriers).
-// Per 128-key tile and warpgroup:  S = Q K^T (8 x wgmma m64n128k16, both operands from shared memory, fp32 in
+// Per 128-key tile and warpgroup:  S = Q K^T (HD / 16 x wgmma m64n128k16, both operands from shared memory, fp32 in
 //                    registers) -> hidden keys to -inf (one 32-bit visibility word per 32 keys), online softmax in
 //                    fp32 -> P (bf16 pairs) stays in registers: the S accumulator layout is the A-fragment layout of
-//                    -> O += P V (8 x wgmma m64n128k16, A from registers, V consumed MN-major straight from the
+//                    -> O += P V (8 x wgmma m64n{HD}k16, A from registers, V consumed MN-major straight from the
 //                    TMA tile).  The producer keeps the next tile's K/V in flight while a tile is computed.
+// The kernel is a template on the head dim HD (64 or 128; the plan picks the instance): a 128-row operand tile is
+// HD / 64 SWIZZLE_128B sub-tiles of 64 bf16 columns (one TMA box each), and the O accumulator holds HD / 2 fp32.
 // The KV range is split across the CTAs of a thread-block cluster (one wave of clusters, split count decided on the
 // device from the live length): a single-split CTA normalises and writes bf16 directly; otherwise every thread
 // pushes its partial rows (acc, m, l) into the shared memory of the CTA that owns the row (DSMEM) and each CTA
@@ -36,22 +38,29 @@ namespace pia {
 namespace attn {
 
 constexpr int BN = 128;      // keys per tile (wgmma N of QK^T, K extent of PV)
-constexpr int HD = 128;      // head dim
 constexpr int NSTAGE = 2;
 constexpr int NTHREADS = 288;   // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int PRODUCER_WARP = 8;
 constexpr int SUB = 128 * 128;             // bytes of one [128 rows x 64 bf16] swizzle-128B sub-tile
-constexpr int TILE_BYTES = 2 * SUB;        // one 128 x 128 bf16 operand tile
-constexpr int SMEM_Q = 0, SMEM_K = TILE_BYTES, SMEM_V = SMEM_K + NSTAGE * TILE_BYTES;
-constexpr int SMEM_BAR = SMEM_V + NSTAGE * TILE_BYTES;
-constexpr int MRG_ACC = 0;                        // [n_split * RS][128] fp32 partial rows pushed by the cluster (over dead Q/KV tiles)
-constexpr int MRG_ML = 112 * 1024;                // [n_split * RS] (m, l) pairs
-// merge buffers that never alias a live tile (used when the CTA's rows fit: <= 64 rows): peers may push their
-// partial rows as soon as they are done, without first waiting for this CTA to leave its tile loop
-constexpr int MRG_DED_ACC = SMEM_BAR + 256, MRG_DED_ACC_BYTES = (64 + 8) * 128 * 4,  // ns * ceil(64 / ns) <= 64 + MAX_SPLIT - 1 rows
-               MRG_DED_ML = MRG_DED_ACC + MRG_DED_ACC_BYTES;
-constexpr int SMEM_TOTAL = MRG_DED_ML + 1024 + 1024;  // + alignment slack
 constexpr int MAX_SPLIT = 8;            // KV splits per head group (merge keeps all partial rows in flight)
+
+// Shared-memory layout of the head-dim HD instance (HD = 128: two sub-tiles per operand tile, HD = 64: one)
+template <int HD>
+struct Smem {
+  static constexpr int TILE_BYTES = HD / 64 * SUB;  // one 128 x HD bf16 operand tile
+  static constexpr int Q = 0, K = TILE_BYTES, V = K + NSTAGE * TILE_BYTES;
+  static constexpr int BAR = V + NSTAGE * TILE_BYTES;
+  static constexpr int MRG_ACC = 0;                  // [HD / 4 chunks][128 + MAX_SPLIT] float4 partial rows pushed by the cluster (over dead Q/KV tiles)
+  static constexpr int MRG_ML = 7 * TILE_BYTES / 2;  // [n_split * RS] (m, l) pairs (112 KB at HD = 128)
+  // merge buffers that never alias a live tile (used when the CTA's rows fit: <= 64 rows): peers may push their
+  // partial rows as soon as they are done, without first waiting for this CTA to leave its tile loop
+  static constexpr int DED_ACC = BAR + 256, DED_ACC_BYTES = (64 + MAX_SPLIT) * HD * 4,  // ns * ceil(64 / ns) <= 64 + MAX_SPLIT - 1 rows
+                       DED_ML = DED_ACC + DED_ACC_BYTES;
+  static constexpr int TOTAL = DED_ML + 1024 + 1024;  // + alignment slack
+  // the aliased merge area lies inside the Q / K / V tiles, which are dead once every CTA has left its tile loop
+  static_assert(MRG_ACC + HD / 4 * (128 + MAX_SPLIT) * 16 <= MRG_ML, "aliased partial rows overlap the (m, l) pairs");
+  static_assert(MRG_ML + (128 + MAX_SPLIT) * 8 <= BAR, "aliased merge area reaches the barriers");
+};
 
 // ------------------------------------------------------------------------------------------------ PTX
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -86,9 +95,10 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 // registers a wgmma reads or writes asynchronously: pins every later access after the wait above
-__device__ __forceinline__ void fence_regs(float (&d)[64]) {
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
 #pragma unroll
-  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 __device__ __forceinline__ void fence_regs(uint32_t (&a)[32]) {
 #pragma unroll
@@ -111,6 +121,16 @@ __device__ __forceinline__ void wgmma_pv(float (&d)[64], const uint32_t *a, uint
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, 1, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b)
+      : "memory");
+}
+// D[64 x 64] += P[64 x 16] V[16 x 64]: the head-dim-64 PV (one V sub-tile)
+__device__ __forceinline__ void wgmma_pv(float (&d)[32], const uint32_t *a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b)
       : "memory");
 }
@@ -200,8 +220,15 @@ __device__ __forceinline__ HeadGroup head_group(const Params &p, int group) {
 
 #define DBG(ev) do { if (p.dbg) p.dbg[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 16 + (ev)] = gtime(); } while (0)
 
+template <int HD>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, Params p) {
+  constexpr int TILE_BYTES = Smem<HD>::TILE_BYTES, SMEM_Q = Smem<HD>::Q, SMEM_K = Smem<HD>::K, SMEM_V = Smem<HD>::V;
+  constexpr int SMEM_BAR = Smem<HD>::BAR, MRG_ACC = Smem<HD>::MRG_ACC, MRG_ML = Smem<HD>::MRG_ML;
+  constexpr int MRG_DED_ACC = Smem<HD>::DED_ACC, MRG_DED_ACC_BYTES = Smem<HD>::DED_ACC_BYTES, MRG_DED_ML = Smem<HD>::DED_ML;
+  // staging splits a head row into two halves (the RoPE rotation pairs them) of CH 16-byte chunks; in the K-major
+  // SWIZZLE_128B tile of 64-wide sub-tiles, half h starts h * HALF_SUB bytes and h * HALF_CH chunks into its rows
+  constexpr int CH = HD / 16, HALF_SUB = HD == 128 ? SUB : 0, HALF_CH = HD == 128 ? 0 : CH;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
@@ -300,12 +327,12 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         if (!fused && !waited && key0 + BN > p_safe) { pdl_wait(); waited = true; }
         mbar_wait(bar_kv_empty + 8 * s, ph ^ 1);
         const uint32_t kd = base + SMEM_K + s * TILE_BYTES, vd = base + SMEM_V + s * TILE_BYTES;
-        mbar_expect_tx(bar_kv_full + 8 * s, TILE_BYTES);
-        tma_load_3d(kd, &map_k, bar_kv_full + 8 * s, 0, key0, plane);
-        tma_load_3d(kd + SUB, &map_k, bar_kv_full + 8 * s, 64, key0, plane);
+        mbar_expect_tx(bar_kv_full + 8 * s, TILE_BYTES);  // one 64-wide box per sub-tile
+#pragma unroll
+        for (int b = 0; b < HD / 64; ++b) tma_load_3d(kd + b * SUB, &map_k, bar_kv_full + 8 * s, 64 * b, key0, plane);
         mbar_expect_tx(bar_v_full + 8 * s, TILE_BYTES);
-        tma_load_3d(vd, &map_v, bar_v_full + 8 * s, 0, key0, plane);
-        tma_load_3d(vd + SUB, &map_v, bar_v_full + 8 * s, 64, key0, plane);
+#pragma unroll
+        for (int b = 0; b < HD / 64; ++b) tma_load_3d(vd + b * SUB, &map_v, bar_v_full + 8 * s, 64 * b, key0, plane);
         if (i == 0) DBG(2);
       }
     }
@@ -313,20 +340,20 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
     if (ns > 1) { barrier_a(); cluster_sync_all(); }
   } else {
     pdl_wait();  // Q (or, fused, the projection output) below is the predecessor's output
-    // ================================================================ staging: thread = (tile row srow, 64-wide half)
+    // ================================================================ staging: thread = (tile row srow, HD / 2-wide half)
     {
       const int srow = tid & 127, half = tid >> 7;
       const int hs = srow / p.np, node = srow % p.np;
       if (srow < rows_used) {
         if (!fused) {
-          uint4 qv[8];  // Q row -> shared memory (K-major SWIZZLE_128B); each half loads one 64-wide d sub-tile
+          uint4 qv[CH];  // Q row -> shared memory (K-major SWIZZLE_128B); each half loads HD / 2 elements of d
           const bool have = hs < heads_here && node < n;
-          const uint4 *src = reinterpret_cast<const uint4 *>(p.q + ((row0 + node) * p.n_q_heads + hq0 + hs) * HD) + half * 8;
+          const uint4 *src = reinterpret_cast<const uint4 *>(p.q + ((row0 + node) * p.n_q_heads + hq0 + hs) * HD) + half * CH;
 #pragma unroll
-          for (int ch = 0; ch < 8; ++ch) qv[ch] = have ? src[ch] : make_uint4(0, 0, 0, 0);
+          for (int ch = 0; ch < CH; ++ch) qv[ch] = have ? src[ch] : make_uint4(0, 0, 0, 0);
 #pragma unroll
-          for (int ch = 0; ch < 8; ++ch)
-            *reinterpret_cast<uint4 *>(sm + SMEM_Q + half * SUB + srow * 128 + ((ch ^ (srow & 7)) << 4)) = qv[ch];
+          for (int ch = 0; ch < CH; ++ch)
+            *reinterpret_cast<uint4 *>(sm + SMEM_Q + half * HALF_SUB + srow * 128 + (((half * HALF_CH + ch) ^ (srow & 7)) << 4)) = qv[ch];
         } else {
           unsigned long long mr0 = 0ull, mr1 = 0ull;
           if (node < n) {
@@ -344,11 +371,11 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
           // All global loads of a batch are issued (read-only path: the compiler may not move plain loads across the
           // shared memory stores in between, and eight dependent load rounds would serialise the prologue) before the
           // first value is used; four 16-byte chunks per batch bound the registers.
-          {  // Q: rotate this thread's 64-wide half (the other half of the head is the rotation partner)
-            const uint4 *qa = reinterpret_cast<const uint4 *>(xr + (long long)(hq0 + hs) * HD) + half * 8;
-            const uint4 *qb = reinterpret_cast<const uint4 *>(xr + (long long)(hq0 + hs) * HD) + (half ^ 1) * 8;
+          {  // Q: rotate this thread's half (the other half of the head is the rotation partner)
+            const uint4 *qa = reinterpret_cast<const uint4 *>(xr + (long long)(hq0 + hs) * HD) + half * CH;
+            const uint4 *qb = reinterpret_cast<const uint4 *>(xr + (long long)(hq0 + hs) * HD) + (half ^ 1) * CH;
 #pragma unroll
-            for (int b4 = 0; b4 < 2; ++b4) {
+            for (int b4 = 0; b4 < CH / 4; ++b4) {
               uint4 ra[4], rb[4], rc[4], rs[4];
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
@@ -359,7 +386,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
               for (int j = 0; j < 4; ++j) {
                 const int ch = b4 * 4 + j;
                 const uint4 o = have ? rope8(ra[j], rb[j], rc[j], rs[j], half == 0) : make_uint4(0, 0, 0, 0);
-                *reinterpret_cast<uint4 *>(sm + SMEM_Q + half * SUB + srow * 128 + ((ch ^ (srow & 7)) << 4)) = o;
+                *reinterpret_cast<uint4 *>(sm + SMEM_Q + half * HALF_SUB + srow * 128 + (((half * HALF_CH + ch) ^ (srow & 7)) << 4)) = o;
               }
             }
           }
@@ -370,13 +397,13 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
             // the reference's torch.cat of past and new K/V, modeling_llama.py:265-268)
             const bool key_row = hs == 0 && node < n;
             const bool writer = hg.j == 0;  // the first head group of the KV head (hq0 % G == 0)
-            const uint4 *ka = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + half * 8;
-            const uint4 *kb = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + (half ^ 1) * 8;
-            const uint4 *va = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + p.n_kv_heads + hkv) * HD) + half * 8;
-            const long long crow = (long long)slot * p.sl.kv_slot_stride + ((long long)hkv * p.max_seq + P + node) * HD + half * 64;
+            const uint4 *ka = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + half * CH;
+            const uint4 *kb = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + hkv) * HD) + (half ^ 1) * CH;
+            const uint4 *va = reinterpret_cast<const uint4 *>(xr + (long long)(p.n_q_heads + p.n_kv_heads + hkv) * HD) + half * CH;
+            const long long crow = (long long)slot * p.sl.kv_slot_stride + ((long long)hkv * p.max_seq + P + node) * HD + half * (HD / 2);
             uint4 *kdst = reinterpret_cast<uint4 *>(p.kc_layer + crow), *vdst = reinterpret_cast<uint4 *>(p.vc_layer + crow);
 #pragma unroll
-            for (int b4 = 0; b4 < 2; ++b4) {
+            for (int b4 = 0; b4 < CH / 4; ++b4) {
               uint4 ra[4], rb[4], rc[4], rs[4], rv[4];
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
@@ -389,7 +416,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
                 const int ch = b4 * 4 + j;
-                const uint32_t off = half * SUB + srow * 128 + ((ch ^ (srow & 7)) << 4);
+                const uint32_t off = half * HALF_SUB + srow * 128 + (((half * HALF_CH + ch) ^ (srow & 7)) << 4);
                 uint4 ko = make_uint4(0, 0, 0, 0), vo = make_uint4(0, 0, 0, 0);
                 if (key_row) { ko = rope8(ra[j], rb[j], rc[j], rs[j], half == 0); vo = rv[j]; }
                 *reinterpret_cast<uint4 *>(sm + SMEM_K + off) = ko;
@@ -402,8 +429,8 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
       } else if (has_draft) {
         // rows 64..127 of a 64-row tile: the draft tile's key rows there are never live, they are zeroed
 #pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {
-          const uint32_t off = half * SUB + srow * 128 + ((ch ^ (srow & 7)) << 4);
+        for (int ch = 0; ch < CH; ++ch) {
+          const uint32_t off = half * HALF_SUB + srow * 128 + (((half * HALF_CH + ch) ^ (srow & 7)) << 4);
           *reinterpret_cast<uint4 *>(sm + SMEM_K + off) = make_uint4(0, 0, 0, 0);
           *reinterpret_cast<uint4 *>(sm + SMEM_V + off) = make_uint4(0, 0, 0, 0);
         }
@@ -433,9 +460,9 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         }
       }
       const uint32_t qa = base + SMEM_Q + wg * 64 * 128;
-      float o[64];
+      float o[HD / 2];
 #pragma unroll
-      for (int j = 0; j < 64; ++j) o[j] = 0.f;
+      for (int j = 0; j < HD / 2; ++j) o[j] = 0.f;
       float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // l_run: this thread's 32 columns of the row
       for (int i = 0; i < ntile; ++i) {
         const int tl = tile_of(i);
@@ -539,7 +566,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
           m_run[h] = m_new[h];
         }
 #pragma unroll
-        for (int nb = 0; nb < 16; ++nb) {
+        for (int nb = 0; nb < HD / 8; ++nb) {
           o[4 * nb] *= alpha[0]; o[4 * nb + 1] *= alpha[0];
           o[4 * nb + 2] *= alpha[1]; o[4 * nb + 3] *= alpha[1];
         }
@@ -548,7 +575,8 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         wgmma_fence();
 #pragma unroll
         for (int j = 0; j < BN / 16; ++j) {
-          // B = V, MN-major: 16 keys = 2 groups of 8 rows (SBO 1024 B), d-halves 16 KB apart (LBO)
+          // B = V, MN-major: 16 keys = 2 groups of 8 rows (SBO 1024 B), 64-wide d sub-tiles 16 KB apart (LBO);
+          // wgmma N = HD (the overload taking this o[])
           wgmma_pv(o, pa + 4 * j, make_desc(va + j * 2048, SUB, 1024));
         }
         wgmma_commit();
@@ -576,7 +604,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
             const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
             uint32_t *dst = reinterpret_cast<uint32_t *>(p.out + ((row0 + node[h]) * p.n_q_heads + hl.hq0 + hs[h]) * HD);
 #pragma unroll
-            for (int nb = 0; nb < 16; ++nb) {
+            for (int nb = 0; nb < HD / 8; ++nb) {
               __nv_bfloat162 b = __floats2bfloat162_rn(o[4 * nb + 2 * h] * inv, o[4 * nb + 2 * h + 1] * inv);
               dst[4 * nb + (lane & 3)] = *reinterpret_cast<uint32_t *>(&b);
             }
@@ -594,11 +622,11 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         for (int h = 0; h < 2; ++h) {
           if (live[h]) {
             const int owner = rw[h] / RS, rl = rw[h] % RS;
-            // partial rows are stored chunk-major ([32 float4 chunks][slot]): head-dim element d = 8 nb + 2 (lane % 4)
+            // partial rows are stored chunk-major ([HD / 4 float4 chunks][slot]): head-dim element d = 8 nb + 2 (lane % 4)
             // lies in chunk d / 4 = 2 nb + (lane % 4) / 2, at float offset 2 (lane % 2)
             const uint32_t dst = map_to_cta(base + mrg_acc + (uint32_t)((((lane & 3) >> 1) * mrg_stride + split * RS + rl) * 16 + (lane & 1) * 8), owner);
 #pragma unroll
-            for (int nb = 0; nb < 16; ++nb)
+            for (int nb = 0; nb < HD / 8; ++nb)
               st_cluster_f2(dst + (uint32_t)(2 * nb * mrg_stride) * 16, o[4 * nb + 2 * h], o[4 * nb + 2 * h + 1]);
             if ((lane & 3) == 0) st_cluster_f2(map_to_cta(base + mrg_ml + (uint32_t)(split * RS + rl) * 8, owner), m_run[h], l_run[h]);
           }
@@ -701,7 +729,10 @@ static int encode_kv_map(CUtensorMap *m, void *base, const pia_attn_config_t &c)
 extern "C" int pia_attn_plan_create(const pia_attn_config_t *cfg, void *d_k_cache, void *d_v_cache,
                                     pia_attn_plan_t **out) {
   PIA_REQUIRE(cfg && d_k_cache && d_v_cache && out, "null argument");
-  if (cfg->head_dim != HD) { set_error("head_dim %d: only 128 is built in this round", cfg->head_dim); return PIA_ERR_UNSUPPORTED; }
+  if (cfg->head_dim != 64 && cfg->head_dim != 128) {
+    set_error("head_dim %d: k_tree_attn is built for 64 and 128", cfg->head_dim);
+    return PIA_ERR_UNSUPPORTED;
+  }
   PIA_REQUIRE(cfg->max_nodes == 64 || cfg->max_nodes == 128, "max_nodes must be 64 or 128");
   PIA_REQUIRE(cfg->n_q_heads > 0 && cfg->n_kv_heads > 0 && cfg->n_q_heads % cfg->n_kv_heads == 0, "bad head counts");
   PIA_REQUIRE(cfg->max_seq > 0 && cfg->n_layers > 0, "bad cache shape");
@@ -731,7 +762,9 @@ extern "C" int pia_attn_plan_create(const pia_attn_config_t *cfg, void *d_k_cach
   int rc = encode_kv_map(&p->map_k, d_k_cache, *cfg);
   if (rc == PIA_OK) rc = encode_kv_map(&p->map_v, d_v_cache, *cfg);
   if (rc == PIA_OK) {
-    cudaError_t e = cudaFuncSetAttribute(k_tree_attn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
+    cudaError_t e = cfg->head_dim == 64
+                        ? cudaFuncSetAttribute(k_tree_attn<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<64>::TOTAL)
+                        : cudaFuncSetAttribute(k_tree_attn<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<128>::TOTAL);
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); rc = PIA_ERR_CUDA; }
   }
   p->dbg = nullptr;
@@ -797,10 +830,15 @@ static int attn_launch(pia_attn_plan_t *p, int layer, const void *d_q, const voi
   const long long layer_off = ((long long)slots->kv_first_slot * p->cfg.n_layers + layer) * p->cfg.n_kv_heads *
                               (long long)p->cfg.max_seq * p->cfg.head_dim;
   a.kc_layer = p->k_base + layer_off; a.vc_layer = p->v_base + layer_off;
-  a.scale_log2 = scale_mul * 1.4426950408889634f / sqrtf((float)HD);
+  a.scale_log2 = scale_mul * 1.4426950408889634f / sqrtf((float)p->cfg.head_dim);
   cudaStream_t s = (cudaStream_t)stream;
-  PIA_CUDA_CHECK(launch_kernel_cluster(k_tree_attn, dim3(ns, p->n_groups, slots->batch), dim3(NTHREADS), SMEM_TOTAL, s,
-                                       (unsigned)ns, p->map_k, p->map_v, a));
+  const dim3 grid(ns, p->n_groups, slots->batch);
+  if (p->cfg.head_dim == 64)
+    PIA_CUDA_CHECK(launch_kernel_cluster(k_tree_attn<64>, grid, dim3(NTHREADS), Smem<64>::TOTAL, s, (unsigned)ns,
+                                         p->map_k, p->map_v, a));
+  else
+    PIA_CUDA_CHECK(launch_kernel_cluster(k_tree_attn<128>, grid, dim3(NTHREADS), Smem<128>::TOTAL, s, (unsigned)ns,
+                                         p->map_k, p->map_v, a));
   count_launch();
   return PIA_OK;
 }

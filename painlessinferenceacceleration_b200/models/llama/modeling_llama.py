@@ -10,6 +10,7 @@ The module tree and parameter names are HF's (so checkpoints load unchanged); th
 is never built: `mask` is the per-node ancestor bit set, the prefix is implicit."""
 import glob
 import json
+import math
 import os
 
 import torch
@@ -421,6 +422,9 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
     def geometry(self):
         c = self.config
         hd = c.hidden_size // c.num_attention_heads
+        if getattr(c, 'head_dim', None) not in (None, hd):   # the projections are built hidden_size wide per head set
+            raise ValueError(f'config head_dim {c.head_dim} differs from hidden_size // num_attention_heads = {hd}; '
+                             'only configs where the two are equal are supported')
         return dict(n_layers=c.num_hidden_layers, hidden=c.hidden_size, n_q_heads=c.num_attention_heads,
                     n_kv_heads=getattr(c, 'num_key_value_heads', None) or c.num_attention_heads, head_dim=hd,
                     inter=c.intermediate_size, vocab=c.vocab_size)
@@ -446,6 +450,18 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             if max_pos > mpe:
                 base = theta * ((factor * max_pos / mpe) - (factor - 1)) ** (hd / (hd - 2))
                 inv_freq = 1.0 / (base ** (torch.arange(0, hd, 2, dtype=torch.int64).float().to(dev) / hd))
+        elif rtype == 'llama3':      # Llama 3.1 / 3.2: long wavelengths / factor, a smooth blend between the two bounds
+            # (transformers' _compute_llama3_parameters, op for op, so the bf16 tables come out bit for bit; attention
+            # factor 1)
+            factor, low, high = float(scaling['factor']), float(scaling['low_freq_factor']), float(scaling['high_freq_factor'])
+            old_ctx = scaling.get('original_max_position_embeddings') or c.max_position_embeddings
+            low_freq_wavelen, high_freq_wavelen = old_ctx / low, old_ctx / high
+            wavelen = 2 * math.pi / inv_freq
+            inv_freq_llama = torch.where(wavelen > low_freq_wavelen, inv_freq / factor, inv_freq)
+            smooth_factor = (old_ctx / wavelen - low) / (high - low)
+            smoothed_inv_freq = (1 - smooth_factor) * inv_freq_llama / factor + smooth_factor * inv_freq_llama
+            is_medium_freq = ~(wavelen < high_freq_wavelen) * ~(wavelen > low_freq_wavelen)
+            inv_freq = torch.where(is_medium_freq, smoothed_inv_freq, inv_freq_llama)
         else:                        # the reference raises on unknown types as well (:241 `Unknown RoPE scaling type`)
             raise ValueError(f'Unknown RoPE scaling type {rtype}')
         freqs = pos[:, None] * inv_freq[None, :]
