@@ -292,6 +292,15 @@ int pia_rmsnorm_partials(const float *d_x_parts, int n_parts, int64_t part_strid
 int pia_rope_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
                        int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin, int max_pos,
                        void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq, void *stream);
+/* The same in the GLM layout (ChatGLM2/3, GLM-4; chatglm/modeling_chatglm.py:156-169, positions :815 = rowsum(mask)
+ * - 1): only dims d < rotary_dim of every q / k head rotate, in interleaved pairs (2i, 2i+1) with frequency i; dims
+ * >= rotary_dim are copied unchanged.  d_cos / d_sin : [max_pos, rotary_dim/2] bf16.  Every product and sum is rounded
+ * to bf16 as eager torch does.  rotary_dim must be a positive multiple of 8 and <= head_dim, else PIA_ERR_INVALID
+ * and nothing is launched.  All other arguments as pia_rope_kv_append. */
+int pia_rope_interleaved_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
+                                   int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin,
+                                   int max_pos, void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer,
+                                   int max_seq, int rotary_dim, void *stream);
 /* SiLU(gate) * up (modeling_llama.py:185-186). d_gate_up : [rows, 2*inter] (gate | up) -> d_out [rows, inter] */
 int pia_silu_mul(const void *d_gate_up, int rows, int inter, void *d_out, void *stream);
 /* embedding gather for the draft nodes: d_out[i] = table[d_ids[i]] (rows >= *d_n are zero filled) */

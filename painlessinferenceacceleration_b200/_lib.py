@@ -93,6 +93,8 @@ SYMBOLS = {
     'pia_gemm_run': (C.c_int, [vp, C.c_int, vp, vp]),
     'pia_rope_kv_append': (C.c_int, [vp, vp, C.c_int, C.POINTER(Slots), C.c_int, C.c_int, C.c_int, vp, vp,
                                      C.c_int, vp, vp, vp, C.c_int, vp]),
+    'pia_rope_interleaved_kv_append': (C.c_int, [vp, vp, C.c_int, C.POINTER(Slots), C.c_int, C.c_int, C.c_int, vp,
+                                                 vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp]),
     'pia_silu_mul': (C.c_int, [vp, C.c_int, C.c_int, vp, vp]),
     'pia_embed_gather': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     'pia_moe_combine': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),

@@ -224,13 +224,20 @@ class Slots(object):
         return C.byref(self.c)
 
 
-def rope_kv_append(qkv, mask, slots, n_q_heads, n_kv_heads, head_dim, cos, sin, q_out, k_layer, v_layer, max_seq):
+def rope_kv_append(qkv, mask, slots, n_q_heads, n_kv_heads, head_dim, cos, sin, q_out, k_layer, v_layer, max_seq,
+                   rotary_dim=None):
     """qkv / q_out: >= slots.rows rows; mask: [>= slots.rows, W] int64 ancestor rows; k_layer / v_layer: the layer's
-    [n_kv_heads, max_seq, head_dim] planes of slot 0"""
+    [n_kv_heads, max_seq, head_dim] planes of slot 0.  rotary_dim=None: Llama RoPE over the whole head (tables
+    [max_pos, head_dim/2]); an int: GLM RoPE, interleaved pairs over the first rotary_dim dims (tables
+    [max_pos, rotary_dim/2]), the rest passed through (pia_rope_interleaved_kv_append)"""
     assert qkv.shape[0] >= slots.rows and mask.shape[0] >= slots.rows
-    L.check(L.load().pia_rope_kv_append(_p(qkv), _p(mask), mask.shape[-1], slots.ref(), n_q_heads, n_kv_heads,
-                                        head_dim, _p(cos), _p(sin), cos.shape[0], _p(q_out), _p(k_layer), _p(v_layer),
-                                        max_seq, _s()))
+    L_ = L.load()
+    args = (_p(qkv), _p(mask), mask.shape[-1], slots.ref(), n_q_heads, n_kv_heads, head_dim, _p(cos), _p(sin),
+            cos.shape[0], _p(q_out), _p(k_layer), _p(v_layer), max_seq)
+    if rotary_dim is None:
+        L.check(L_.pia_rope_kv_append(*args, _s()))
+    else:
+        L.check(L_.pia_rope_interleaved_kv_append(*args, int(rotary_dim), _s()))
 
 
 def silu_mul(gate_up, out):

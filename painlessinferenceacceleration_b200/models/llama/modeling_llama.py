@@ -117,10 +117,14 @@ class LlamaDecoderLayer(nn.Module):
 
     def __init__(self, cfg, device, dtype):
         super().__init__()
-        self.self_attn = LlamaAttention(cfg, device, dtype, qkv_bias=self.qkv_bias)
+        self.self_attn = LlamaAttention(cfg, device, dtype, qkv_bias=self._qkv_bias(cfg))
         self.mlp = self._make_mlp(cfg, device, dtype)
         self.input_layernorm = LlamaRMSNorm(cfg.hidden_size, cfg.rms_norm_eps, device, dtype)
         self.post_attention_layernorm = LlamaRMSNorm(cfg.hidden_size, cfg.rms_norm_eps, device, dtype)
+
+    def _qkv_bias(self, cfg):
+        """whether q/k/v carry biases: the class's flag (a family may read it from the config instead)"""
+        return self.qkv_bias
 
     def _make_mlp(self, cfg, device, dtype):
         return LlamaMLP(cfg, device, dtype)
@@ -138,6 +142,8 @@ class LlamaModel(nn.Module):
 
 class LlamaForCausalLM(LookaheadPreTrainedModel):
     model_cls = LlamaModel
+    rotary_interleaved = False   # GLM: RoPE on the first geometry()['rotary_dim'] dims of a head, in (2i, 2i+1) pairs
+    sandwich_norms = False       # GLM-4-0414: RMSNorm of each sublayer's output before its residual add
 
     def __init__(self, config, device=None, dtype=torch.bfloat16):
         super().__init__(config)
@@ -177,10 +183,9 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         """HF checkpoint directory (config.json + *.safetensors / pytorch_model*.bin) -> model on the GPU.
         quantization='fp8': the decoder projections become fp8 weights as they arrive (see quantize_fp8); the bf16
         decoder never exists on the GPU."""
-        from transformers import AutoConfig
         if quantization not in (None, 'fp8'):
             raise ValueError(f'quantization={quantization!r}: only None and \'fp8\' are supported')
-        config = AutoConfig.from_pretrained(path)
+        config = cls._pretrained_config(path)
         if quantization == 'fp8':
             return cls._from_pretrained_fp8(path, config, device)
         model = cls(config, device=device, dtype=torch_dtype)
@@ -201,6 +206,12 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         if missing:
             raise RuntimeError(f'checkpoint is missing {len(missing)} tensors, e.g. {missing[:4]}')
         return model
+
+    @classmethod
+    def _pretrained_config(cls, path):
+        """the config of a checkpoint directory (HF format: AutoConfig)"""
+        from transformers import AutoConfig
+        return AutoConfig.from_pretrained(path)
 
     # the parameters of a decoder layer that fp8 mode quantises (relative to the layer)
     _fp8_params = ('self_attn.q_proj.weight', 'self_attn.k_proj.weight', 'self_attn.v_proj.weight',
@@ -578,6 +589,12 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                     ops.l2_prefetch(t, range_bytes=int(total * min(frac, 1.0)) // 16 * 16, gbytes_per_s=pf['rate'])
         pf['dirty'] = True
 
+    def _check_fused_attn(self):
+        """the fused RoPE-inside-attention kernel (PIA_ATTN_FUSED) rotates in the half-split layout only"""
+        if self.rotary_interleaved and os.environ.get('PIA_ATTN_FUSED', '0') != '0':
+            raise ValueError(f'{type(self).__name__} rotates interleaved pairs (GLM RoPE), which the fused attention '
+                             'kernel does not: unset PIA_ATTN_FUSED')
+
     # ------------------------------------------------------------------ the verify forward on static buffers
     def _mlp(self, rt, layer, y, plans=None, pf=None, b=None):
         """returns (x, parts): the MLP output as a bf16 tensor or as fp32 split-K slices for the next rmsnorm.
@@ -623,6 +640,9 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         pf = self._prefetch_cfg(rt) if plans and not self._fp8 else False
         fused_attn = b is rt.decode_bufs and os.environ.get('PIA_ATTN_FUSED', '0') != '0' and \
             (b.slots.batch == 1 or b.slots.kv_slot_stride != 0)
+        if fused_attn:
+            self._check_fused_attn()
+        rotary_dim = g['rotary_dim'] if self.rotary_interleaved else None
         x, parts, resid_in = b.h, None, None  # norm(x | parts, resid_in) -> (resid = x + resid_in, y = norm(resid))
 
         def norm(w):
@@ -630,6 +650,13 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                 ops.rmsnorm_partials(parts, resid_in, w, eps, b.resid, b.y)
             else:
                 ops.rmsnorm(x, resid_in, w, eps, b.resid, b.y)
+
+        def post_norm(w):   # a sublayer output normalised alone (no residual), into b.post_norm
+            if parts is not None:
+                ops.rmsnorm_partials(parts, None, w, eps, None, b.post_norm)
+            else:
+                ops.rmsnorm(x, None, w, eps, None, b.post_norm)
+            return b.post_norm, None
 
         for li, layer in enumerate(self.model.layers):
             lp = plans['layers'][li] if plans else None
@@ -650,15 +677,20 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                 rt.plan.forward_fused(li, b.qkv, b.mask, b.slots, rt.rope_cos, rt.rope_sin, b.attn)
             else:            # prefill chunks share one cache: append first, then attend
                 ops.rope_kv_append(b.qkv, b.mask, b.slots, g['n_q_heads'], g['n_kv_heads'], g['head_dim'], rt.rope_cos,
-                                   rt.rope_sin, b.q, rt.k_layer(li, b.kv_slot), rt.v_layer(li, b.kv_slot), rt.max_seq)
+                                   rt.rope_sin, b.q, rt.k_layer(li, b.kv_slot), rt.v_layer(li, b.kv_slot), rt.max_seq,
+                                   rotary_dim=rotary_dim)
                 rt.plan.forward(li, b.q, b.mask, b.slots, b.attn)
             if lp and 'o' in lp:
                 o = lp['o'].run(rows)
                 x, parts, resid_in = (o, None, b.resid) if lp['o'].splits == 1 else (None, o, b.resid)
             else:
                 x, parts, resid_in = torch.mm(b.attn, a.o_proj.weight.t()), None, b.resid
+            if self.sandwich_norms:
+                x, parts = post_norm(layer.post_self_attn_layernorm.weight)
             norm(layer.post_attention_layernorm.weight)
             x, parts = self._mlp(rt, layer, b.y, lp, pf, b=b)
+            if self.sandwich_norms:
+                x, parts = post_norm(layer.post_mlp_layernorm.weight)
         if pf and pf.pop('dirty', False):  # join the side stream (required before a capture ends)
             torch.cuda.current_stream().wait_stream(pf['side'])
         if last_only:
