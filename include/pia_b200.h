@@ -223,6 +223,15 @@ int pia_tree_attn_fused_fwd(pia_attn_plan_t *p, int layer, const void *d_qkv, co
                             int max_pos, const uint64_t *d_mask, const pia_slots_t *slots, float scale_mul, void *d_out,
                             void *stream);
 
+/* pia_tree_attn_fwd with an ALiBi bias (Baichuan-13B, Baichuan2-13B: baichuan_13b/modeling_baichuan.py:25-36,
+ * :146-157): score = q.k / sqrt(head_dim) * scale_mul + d_slopes[h] * (kpos - qpos), in fp32, hidden keys excluded
+ * as before.  Positions are TREE positions (the reference's BLOOM patch, bloom/modeling_bloom.py:170): a row at tree
+ * depth t (rowsum(mask) - 1) has qpos = max(P - pad, 0) + t; cached key j < P has kpos = j - pad; draft key k has
+ * kpos = max(P - pad, 0) + depth(k).  d_slopes : [n_q_heads] fp32 device array.  head_dim 128 only (head_dim 64:
+ * PIA_ERR_UNSUPPORTED).  Arguments and capturability otherwise as pia_tree_attn_fwd. */
+int pia_tree_attn_alibi_fwd(pia_attn_plan_t *p, int layer, const void *d_q, const uint64_t *d_mask,
+                            const pia_slots_t *slots, float scale_mul, const float *d_slopes, void *d_out, void *stream);
+
 /* ============================================================================================
  * Weight-streaming GEMM of the verify forward: Y[t, n] = sum_k X[t, k] W[n, k]  (X: <= 64 draft rows, W = an
  * nn.Linear weight [N, K] bf16), i.e. the projections of modeling_llama.py:254-256, :303, :185-186, :769.
@@ -301,6 +310,12 @@ int pia_rope_interleaved_kv_append(const void *d_qkv, const uint64_t *d_mask, in
                                    int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin,
                                    int max_pos, void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer,
                                    int max_seq, int rotary_dim, void *stream);
+/* The same as pia_rope_kv_append with fp32 tables d_cos / d_sin : [max_pos, D/2] float and fp32 arithmetic:
+ * bf16(fp32(x * cos) + fp32(rotate_half(x) * sin)), no FMA contraction, one rounding (Baichuan2-7B,
+ * baichuan2_7b/modeling_baichuan.py:148-155).  All other arguments as pia_rope_kv_append. */
+int pia_rope_f32_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
+                           int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin, int max_pos,
+                           void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq, void *stream);
 /* SiLU(gate) * up (modeling_llama.py:185-186). d_gate_up : [rows, 2*inter] (gate | up) -> d_out [rows, inter] */
 int pia_silu_mul(const void *d_gate_up, int rows, int inter, void *d_out, void *stream);
 /* embedding gather for the draft nodes: d_out[i] = table[d_ids[i]] (rows >= *d_n are zero filled) */

@@ -80,6 +80,7 @@ SYMBOLS = {
     'pia_attn_plan_grid': (C.c_int, [vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'pia_tree_attn_fwd': (C.c_int, [vp, C.c_int, vp, vp, C.POINTER(Slots), C.c_float, vp, vp]),
     'pia_tree_attn_fused_fwd': (C.c_int, [vp, C.c_int, vp, vp, vp, C.c_int, vp, C.POINTER(Slots), C.c_float, vp, vp]),
+    'pia_tree_attn_alibi_fwd': (C.c_int, [vp, C.c_int, vp, vp, C.POINTER(Slots), C.c_float, vp, vp, vp]),
     'pia_rmsnorm': (C.c_int, [vp, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp]),
     'pia_rmsnorm_partials': (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp]),
     'pia_gemm_plan_create': (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
@@ -95,6 +96,8 @@ SYMBOLS = {
                                      C.c_int, vp, vp, vp, C.c_int, vp]),
     'pia_rope_interleaved_kv_append': (C.c_int, [vp, vp, C.c_int, C.POINTER(Slots), C.c_int, C.c_int, C.c_int, vp,
                                                  vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp]),
+    'pia_rope_f32_kv_append': (C.c_int, [vp, vp, C.c_int, C.POINTER(Slots), C.c_int, C.c_int, C.c_int, vp, vp,
+                                         C.c_int, vp, vp, vp, C.c_int, vp]),
     'pia_silu_mul': (C.c_int, [vp, C.c_int, C.c_int, vp, vp]),
     'pia_embed_gather': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     'pia_moe_combine': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),

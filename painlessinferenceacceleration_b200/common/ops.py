@@ -2,6 +2,7 @@
 """Thin typed wrappers over the C ABI (include/pia_b200.h) for torch tensors: raw device pointers + the current
 torch stream, nothing else. Every call is asynchronous and CUDA-graph capturable."""
 import ctypes as C
+import math
 
 import torch
 
@@ -229,15 +230,41 @@ def rope_kv_append(qkv, mask, slots, n_q_heads, n_kv_heads, head_dim, cos, sin, 
     """qkv / q_out: >= slots.rows rows; mask: [>= slots.rows, W] int64 ancestor rows; k_layer / v_layer: the layer's
     [n_kv_heads, max_seq, head_dim] planes of slot 0.  rotary_dim=None: Llama RoPE over the whole head (tables
     [max_pos, head_dim/2]); an int: GLM RoPE, interleaved pairs over the first rotary_dim dims (tables
-    [max_pos, rotary_dim/2]), the rest passed through (pia_rope_interleaved_kv_append)"""
+    [max_pos, rotary_dim/2]), the rest passed through (pia_rope_interleaved_kv_append).  float32 tables (Llama layout
+    only): fp32 arithmetic, one bf16 rounding (pia_rope_f32_kv_append, Baichuan2-7B)"""
     assert qkv.shape[0] >= slots.rows and mask.shape[0] >= slots.rows
+    assert cos.dtype == sin.dtype and cos.dtype in (torch.bfloat16, torch.float32)
     L_ = L.load()
     args = (_p(qkv), _p(mask), mask.shape[-1], slots.ref(), n_q_heads, n_kv_heads, head_dim, _p(cos), _p(sin),
             cos.shape[0], _p(q_out), _p(k_layer), _p(v_layer), max_seq)
-    if rotary_dim is None:
+    if cos.dtype == torch.float32:
+        if rotary_dim is not None:
+            raise ValueError('fp32 RoPE tables exist for the half-split (Llama) layout only')
+        L.check(L_.pia_rope_f32_kv_append(*args, _s()))
+    elif rotary_dim is None:
         L.check(L_.pia_rope_kv_append(*args, _s()))
     else:
         L.check(L_.pia_rope_interleaved_kv_append(*args, int(rotary_dim), _s()))
+
+
+def _alibi_slopes_f64(n):
+    """the ALiBi slopes of n heads as python floats (baichuan_13b/modeling_baichuan.py:25-36 `_get_interleave`, the
+    same numbers as BLOOM's build_alibi_tensor): the geometric series start^(i+1), start = 2^(-8/n), for a power of
+    two n; otherwise that series for the largest power of two c < n, then every other slope of the 2c series"""
+    def pow2(m):
+        start = 2 ** (-(2 ** -(math.log2(m) - 3)))
+        return [start * start ** i for i in range(m)]
+    if math.log2(n).is_integer():
+        return pow2(n)
+    c = 2 ** math.floor(math.log2(n))
+    return pow2(c) + _alibi_slopes_f64(2 * c)[0::2][:n - c]
+
+
+def alibi_slopes(n_heads):
+    """fp32 [n_heads] CPU tensor of the ALiBi slopes, computed in float64 and then cast"""
+    if int(n_heads) < 1:
+        raise ValueError(f'n_heads={n_heads}: ALiBi needs at least one head')
+    return torch.tensor(_alibi_slopes_f64(int(n_heads)), dtype=torch.float64).to(torch.float32)
 
 
 def silu_mul(gate_up, out):
@@ -291,9 +318,18 @@ class AttnPlan(object):
             L.check(self.lib.pia_attn_plan_create(C.byref(self.cfg), _p(k_cache), _p(v_cache), C.byref(self.h)))
         self._keep = (k_cache, v_cache)
 
-    def forward(self, layer, q, mask, slots, out, scale_mul=1.0):
+    def forward(self, layer, q, mask, slots, out, scale_mul=1.0, alibi_slopes=None):
+        """alibi_slopes: None, or an fp32 device tensor [n_q_heads] -> the ALiBi bias at tree positions
+        (pia_tree_attn_alibi_fwd, head_dim 128)"""
         assert q.shape[0] >= slots.rows and mask.shape[0] >= slots.rows and out.shape[0] >= slots.rows
-        L.check(self.lib.pia_tree_attn_fwd(self.h, layer, _p(q), _p(mask), slots.ref(), float(scale_mul), _p(out), _s()))
+        if alibi_slopes is None:
+            L.check(self.lib.pia_tree_attn_fwd(self.h, layer, _p(q), _p(mask), slots.ref(), float(scale_mul), _p(out),
+                                               _s()))
+            return
+        assert alibi_slopes.dtype == torch.float32 and alibi_slopes.numel() == self.cfg.n_q_heads and \
+            alibi_slopes.is_cuda and alibi_slopes.is_contiguous()
+        L.check(self.lib.pia_tree_attn_alibi_fwd(self.h, layer, _p(q), _p(mask), slots.ref(), float(scale_mul),
+                                                 _p(alibi_slopes), _p(out), _s()))
 
     def forward_fused(self, layer, qkv, mask, slots, cos, sin, out, scale_mul=1.0):
         """RoPE + KV append + tree attention in one launch (pia_tree_attn_fused_fwd): qkv is the fused projection

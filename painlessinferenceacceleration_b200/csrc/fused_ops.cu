@@ -2,7 +2,8 @@
 //   k_rmsnorm           models/llama/modeling_llama.py:76-90   (+ the residual add of the decoder layer :340-352)
 //   k_rope_kv_append    :156-169 apply_rotary_pos_emb at the tree positions of :587, and the KV-cache append
 //                       that replaces the reference's per-step torch.cat (:265-268); a second instance rotates in
-//                       the GLM layout (chatglm/modeling_chatglm.py:156-169, positions :815)
+//                       the GLM layout (chatglm/modeling_chatglm.py:156-169, positions :815), a third one in fp32
+//                       with fp32 tables (baichuan2_7b/modeling_baichuan.py:148-155)
 //   k_silu_mul          :185-186
 //   k_embed_gather      :582
 // Rounding points follow the reference's bf16 eager arithmetic (each torch op rounds to bf16) so that
@@ -96,15 +97,18 @@ __global__ void __launch_bounds__(512) k_rmsnorm(const __nv_bfloat16 *x, const f
 }
 
 // grid = batch * rows_per_slot rows (pia_slots_t); thread = one (head, 8-wide d chunk) of q | k | v
-// kInterleaved = false: Llama layout, x[d] pairs with x[d +- hd/2] over the whole head, tables [max_pos, hd/2]
-//                       (rotary_dim unused).
-// kInterleaved = true:  GLM layout (chatglm/modeling_chatglm.py:156-169): only d < rotary_dim rotates, in pairs
-//                       (2i, 2i+1) with frequency i, tables [max_pos, rotary_dim/2]; the other dims pass through.
-template <bool kInterleaved>
+// ROPE_HALF:        Llama layout, x[d] pairs with x[d +- hd/2] over the whole head, bf16 tables [max_pos, hd/2]
+//                   (rotary_dim unused).
+// ROPE_INTERLEAVED: GLM layout (chatglm/modeling_chatglm.py:156-169): only d < rotary_dim rotates, in pairs
+//                   (2i, 2i+1) with frequency i, bf16 tables [max_pos, rotary_dim/2]; the other dims pass through.
+// ROPE_HALF_F32:    Llama layout with fp32 tables [max_pos, hd/2] and fp32 arithmetic, one bf16 rounding at the end
+//                   (baichuan2_7b/modeling_baichuan.py:148-155: q.float() * cos + rotate_half(q.float()) * sin).
+enum { ROPE_HALF = 0, ROPE_INTERLEAVED = 1, ROPE_HALF_F32 = 2 };
+template <int kLayout>
 __global__ void __launch_bounds__(256) k_rope_kv_append(const __nv_bfloat16 *qkv, const unsigned long long *mask,
                                                         int mask_words, pia_slots_t sl,
-                                                        int hq, int hkv, int hd, const __nv_bfloat16 *cos_t,
-                                                        const __nv_bfloat16 *sin_t, int max_pos, __nv_bfloat16 *q_out,
+                                                        int hq, int hkv, int hd, const void *cos_t,
+                                                        const void *sin_t, int max_pos, __nv_bfloat16 *q_out,
                                                         __nv_bfloat16 *kc, __nv_bfloat16 *vc, int max_seq,
                                                         int rotary_dim) {
   pdl_launch_dependents();
@@ -133,13 +137,15 @@ __global__ void __launch_bounds__(256) k_rope_kv_append(const __nv_bfloat16 *qkv
     Pack8 a; a.u = *reinterpret_cast<const uint4 *>(src + head * hd + d0);
     if (head < hq + hkv) {  // q or k: x*cos + rotate_half(x)*sin, every product/sum rounded to bf16 like eager torch
       Pack8 o;
-      if constexpr (kInterleaved) {
+      const __nv_bfloat16 *cos_b = static_cast<const __nv_bfloat16 *>(cos_t);
+      const __nv_bfloat16 *sin_b = static_cast<const __nv_bfloat16 *>(sin_t);
+      if constexpr (kLayout == ROPE_INTERLEAVED) {
         o = a;
         if (d0 < rotary_dim) {  // 4 whole pairs (2i, 2i+1), i = d0/2 .. d0/2+3: cos/sin are one 8-byte load each
           const int rhalf = rotary_dim >> 1;
           union { uint2 u; __nv_bfloat16 h[4]; } cs, sn;
-          cs.u = *reinterpret_cast<const uint2 *>(cos_t + (long long)pos * rhalf + (d0 >> 1));
-          sn.u = *reinterpret_cast<const uint2 *>(sin_t + (long long)pos * rhalf + (d0 >> 1));
+          cs.u = *reinterpret_cast<const uint2 *>(cos_b + (long long)pos * rhalf + (d0 >> 1));
+          sn.u = *reinterpret_cast<const uint2 *>(sin_b + (long long)pos * rhalf + (d0 >> 1));
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const float x0 = __bfloat162float(a.h[2 * j]), x1 = __bfloat162float(a.h[2 * j + 1]);
@@ -148,13 +154,29 @@ __global__ void __launch_bounds__(256) k_rope_kv_append(const __nv_bfloat16 *qkv
             o.h[2 * j + 1] = __float2bfloat16_rn(bf(x1 * c) + bf(x0 * s));
           }
         }
+      } else if constexpr (kLayout == ROPE_HALF_F32) {
+        const int dp = d0 < half ? d0 + half : d0 - half;
+        Pack8 b; b.u = *reinterpret_cast<const uint4 *>(src + head * hd + dp);
+        const float *cf = static_cast<const float *>(cos_t) + (long long)pos * half + d0 % half;
+        const float *sf = static_cast<const float *>(sin_t) + (long long)pos * half + d0 % half;
+        float c[8], s[8];
+        *reinterpret_cast<float4 *>(c) = *reinterpret_cast<const float4 *>(cf);
+        *reinterpret_cast<float4 *>(c + 4) = *reinterpret_cast<const float4 *>(cf + 4);
+        *reinterpret_cast<float4 *>(s) = *reinterpret_cast<const float4 *>(sf);
+        *reinterpret_cast<float4 *>(s + 4) = *reinterpret_cast<const float4 *>(sf + 4);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {  // fp32 products and sum, no FMA contraction, one rounding to bf16
+          const float x = __bfloat162float(a.h[j]);
+          const float r = d0 < half ? -__bfloat162float(b.h[j]) : __bfloat162float(b.h[j]);
+          o.h[j] = __float2bfloat16_rn(__fadd_rn(__fmul_rn(x, c[j]), __fmul_rn(r, s[j])));
+        }
       } else {
         const int dp = d0 < half ? d0 + half : d0 - half;
         Pack8 b; b.u = *reinterpret_cast<const uint4 *>(src + head * hd + dp);
         Pack8 cs, sn;
         const int f0 = d0 % half;
-        cs.u = *reinterpret_cast<const uint4 *>(cos_t + (long long)pos * half + f0);
-        sn.u = *reinterpret_cast<const uint4 *>(sin_t + (long long)pos * half + f0);
+        cs.u = *reinterpret_cast<const uint4 *>(cos_b + (long long)pos * half + f0);
+        sn.u = *reinterpret_cast<const uint4 *>(sin_b + (long long)pos * half + f0);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float x = __bfloat162float(a.h[j]);
@@ -230,7 +252,7 @@ extern "C" int pia_rmsnorm_partials(const float *d_x_parts, int n_parts, int64_t
   return PIA_OK;
 }
 
-template <bool kInterleaved>
+template <int kLayout>
 static int rope_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
                           int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin, int max_pos,
                           void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq, int rotary_dim,
@@ -239,10 +261,10 @@ static int rope_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_wo
                   d_k_cache_layer && d_v_cache_layer, "null argument");
   PIA_REQUIRE(slots->batch >= 1 && slots->rows_per_slot >= 1 && slots->kv_slot_stride >= 0, "bad slot table");
   PIA_REQUIRE(head_dim % 16 == 0 && mask_words >= 1 && mask_words <= 2, "bad rope arguments");
-  PIA_CUDA_CHECK(launch_kernel(k_rope_kv_append<kInterleaved>, dim3(slots->batch * slots->rows_per_slot), dim3(256), 0,
+  PIA_CUDA_CHECK(launch_kernel(k_rope_kv_append<kLayout>, dim3(slots->batch * slots->rows_per_slot), dim3(256), 0,
                               (cudaStream_t)stream, (const __nv_bfloat16 *)d_qkv, (const unsigned long long *)d_mask,
-                              mask_words, *slots, n_q_heads, n_kv_heads, head_dim, (const __nv_bfloat16 *)d_cos,
-                              (const __nv_bfloat16 *)d_sin, max_pos, (__nv_bfloat16 *)d_q_out,
+                              mask_words, *slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin, max_pos,
+                              (__nv_bfloat16 *)d_q_out,
                               (__nv_bfloat16 *)d_k_cache_layer, (__nv_bfloat16 *)d_v_cache_layer, max_seq, rotary_dim));
   count_launch();
   return PIA_OK;
@@ -252,8 +274,16 @@ extern "C" int pia_rope_kv_append(const void *d_qkv, const uint64_t *d_mask, int
                                   int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin,
                                   int max_pos, void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq,
                                   void *stream) {
-  return rope_kv_append<false>(d_qkv, d_mask, mask_words, slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin, max_pos,
-                               d_q_out, d_k_cache_layer, d_v_cache_layer, max_seq, head_dim, stream);
+  return rope_kv_append<ROPE_HALF>(d_qkv, d_mask, mask_words, slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin,
+                                   max_pos, d_q_out, d_k_cache_layer, d_v_cache_layer, max_seq, head_dim, stream);
+}
+
+extern "C" int pia_rope_f32_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
+                                      int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin,
+                                      int max_pos, void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer,
+                                      int max_seq, void *stream) {
+  return rope_kv_append<ROPE_HALF_F32>(d_qkv, d_mask, mask_words, slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin,
+                                       max_pos, d_q_out, d_k_cache_layer, d_v_cache_layer, max_seq, head_dim, stream);
 }
 
 extern "C" int pia_rope_interleaved_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words,
@@ -263,7 +293,7 @@ extern "C" int pia_rope_interleaved_kv_append(const void *d_qkv, const uint64_t 
                                               int rotary_dim, void *stream) {
   PIA_REQUIRE(rotary_dim >= 8 && rotary_dim % 8 == 0 && rotary_dim <= head_dim,
               "bad rotary_dim: a positive multiple of 8, at most head_dim");
-  return rope_kv_append<true>(d_qkv, d_mask, mask_words, slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin, max_pos,
+  return rope_kv_append<ROPE_INTERLEAVED>(d_qkv, d_mask, mask_words, slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin, max_pos,
                               d_q_out, d_k_cache_layer, d_v_cache_layer, max_seq, rotary_dim, stream);
 }
 

@@ -43,6 +43,9 @@ constexpr int NTHREADS = 288;   // warps 0-7: two consumer warpgroups, warp 8: T
 constexpr int PRODUCER_WARP = 8;
 constexpr int SUB = 128 * 128;             // bytes of one [128 rows x 64 bf16] swizzle-128B sub-tile
 constexpr int MAX_SPLIT = 8;            // KV splits per head group (merge keeps all partial rows in flight)
+constexpr int ALIBI_SLOPE = 64;         // ALiBi instance, offsets from the barriers: 2 fp32 slopes (one per warpgroup),
+constexpr int ALIBI_DEPTH = 128;        //   and the uint8 depth of each draft node
+constexpr float LOG2E = 1.4426950408889634f;
 
 // Shared-memory layout of the head-dim HD instance (HD = 128: two sub-tiles per operand tile, HD = 64: one)
 template <int HD>
@@ -60,6 +63,9 @@ struct Smem {
   // the aliased merge area lies inside the Q / K / V tiles, which are dead once every CTA has left its tile loop
   static_assert(MRG_ACC + HD / 4 * (128 + MAX_SPLIT) * 16 <= MRG_ML, "aliased partial rows overlap the (m, l) pairs");
   static_assert(MRG_ML + (128 + MAX_SPLIT) * 8 <= BAR, "aliased merge area reaches the barriers");
+  // the ALiBi depths (one byte per draft key) sit between the 3 x NSTAGE barriers and the dedicated merge buffers
+  static_assert(3 * NSTAGE * 8 <= ALIBI_SLOPE && ALIBI_SLOPE + 8 <= ALIBI_DEPTH && BAR + ALIBI_DEPTH + 128 <= DED_ACC,
+                "ALiBi slopes / depths overlap");
 };
 
 // ------------------------------------------------------------------------------------------------ PTX
@@ -198,6 +204,7 @@ struct Params {
   __nv_bfloat16 *kc_layer, *vc_layer;  // this layer's [Hkv, max_seq, HD] planes of the cache slot 0 addresses
   __nv_bfloat16 *out;            // [max_nodes, Hq, HD]
   unsigned long long *dbg;       // optional per-CTA phase timestamps (pia_attn_plan_set_debug)
+  const float *slopes;           // ALiBi instance (pia_tree_attn_alibi_fwd): [Hq] fp32 slopes
 };
 
 __device__ __forceinline__ unsigned long long gtime() {
@@ -220,7 +227,12 @@ __device__ __forceinline__ HeadGroup head_group(const Params &p, int group) {
 
 #define DBG(ev) do { if (p.dbg) p.dbg[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 16 + (ev)] = gtime(); } while (0)
 
-template <int HD>
+// kAlibi (HD = 128 only, plain mode only): every score gets the linear position bias slope_h * (kpos - qpos) of ALiBi
+// (baichuan_13b/modeling_baichuan.py:25-36, :146-157) at TREE positions, as the reference's BLOOM patch computes them
+// (bloom/modeling_bloom.py:170): qpos = max(P - pad, 0) + depth(row) - 1, kpos = j - pad for a cached key j < P and
+// max(P - pad, 0) + depth(k) - 1 for draft key k.  The row offset does not change the softmax, so this is the models'
+// absolute slope_h * kpos; the verify logits of every node equal a causal forward over prefix + root-to-node path.
+template <int HD, bool kAlibi>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, Params p) {
   constexpr int TILE_BYTES = Smem<HD>::TILE_BYTES, SMEM_Q = Smem<HD>::Q, SMEM_K = Smem<HD>::K, SMEM_V = Smem<HD>::V;
@@ -260,7 +272,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
   const int hkv = hg.hkv, hq0 = hg.hq0, heads_here = hg.heads;
   // tiles: plain mode = the keys [0, L) of the cache; fused mode = the prefix tiles [0, P) of the cache + ONE draft tile
   // (the n draft keys, rotated and staged in shared memory by the consumer warps of the CTA that owns the last tile)
-  const bool fused = p.fused != 0;
+  const bool fused = !kAlibi && p.fused != 0;
   const int Tp = (P + BN - 1) / BN;
   const int tiles_total = fused ? Tp + 1 : (L + BN - 1) / BN;
   // Work split decided on the device from the live length: tiles_per_cta tiles per CTA (more only when the
@@ -435,6 +447,24 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
           *reinterpret_cast<uint4 *>(sm + SMEM_V + off) = make_uint4(0, 0, 0, 0);
         }
       }
+      if constexpr (kAlibi) {
+        // in the spare bytes after the barriers: the depth popc(mask[k]) of every draft node (the bias of the draft
+        // keys, and of the query rows) and each warpgroup's slope in the log2 domain.  The tile loop reads them back
+        // from shared memory: held in registers through the loop they would spill.
+        if (tid < p.np) {
+          int d = 0;
+          if (tid < n) {
+            d = __popcll(p.mask[(row0 + tid) * p.mask_words]);
+            if (p.mask_words > 1) d += __popcll(p.mask[(row0 + tid) * p.mask_words + 1]);
+          }
+          sm[SMEM_BAR + ALIBI_DEPTH + tid] = (uint8_t)d;
+        }
+        if (tid < 2) {
+          const int hs_wg = tid * 64 / p.np;  // the query head of warpgroup tid (64 rows each)
+          reinterpret_cast<float *>(sm + SMEM_BAR + ALIBI_SLOPE)[tid] =
+              hs_wg < heads_here ? p.slopes[hq0 + hs_wg] * LOG2E : 0.f;
+        }
+      }
       fence_async_smem();  // generic-proxy stores -> visible to the wgmma (async proxy) reads
     }
     asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -454,7 +484,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         hs[h] = rw[h] / p.np; node[h] = rw[h] % p.np;
         live[h] = node[h] < n;
         mrow[h][0] = mrow[h][1] = 0ull;
-        if (live[h]) {
+        if (!kAlibi && live[h]) {  // the ALiBi instance reads the rows again per masked tile (registers)
           mrow[h][0] = p.mask[(row0 + node[h]) * p.mask_words];
           if (p.mask_words > 1) mrow[h][1] = p.mask[(row0 + node[h]) * p.mask_words + 1];
         }
@@ -489,7 +519,11 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
         if (!all_visible) {  // tree / padded / ragged tile: hidden keys -> -inf once, then the dense code
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const unsigned long long m0 = mrow[h][0], m1 = mrow[h][1];
+            unsigned long long m0 = mrow[h][0], m1 = mrow[h][1];
+            if (kAlibi && live[h]) {
+              m0 = p.mask[(row0 + node[h]) * p.mask_words];
+              if (p.mask_words > 1) m1 = p.mask[(row0 + node[h]) * p.mask_words + 1];
+            }
             auto vis32 = [&](int kb) -> uint32_t {
               if (is_draft) {  // key kb - Tp * BN is draft node j0: visible iff it is an ancestor (or the node itself)
                 const int j0 = kb - Tp * BN;
@@ -529,6 +563,41 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
             }
           }
         }
+        if constexpr (kAlibi) {
+          // scores -> log2 domain with the bias: s * scale_log2 + sl2 * (kpos - qpos); hidden keys stay -inf.
+          // sl2 = the warpgroup's slope * log2(e); a row at depth dq sees cached key j at kpos - qpos = j - cq and
+          // draft key k at depth(k) - dq
+          const uint8_t *depth = sm + SMEM_BAR + ALIBI_DEPTH;
+          const float sl2 = reinterpret_cast<const float *>(sm + SMEM_BAR + ALIBI_SLOPE)[wg];
+          int dq[2], cq[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            dq[h] = depth[(wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * h) & (p.np - 1)];  // the row's node
+            cq[h] = pad_len + (P > pad_len ? P - pad_len : 0) - 1 + dq[h];
+          }
+          if (all_visible) {  // cached keys only: the bias is linear in the column, one FMA per score on top
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float rb = sl2 * (float)(tl * BN + 2 * (lane & 3) - cq[h]);
+#pragma unroll
+              for (int nb = 0; nb < 16; ++nb) {
+                sv[4 * nb + 2 * h] = fmaf(sv[4 * nb + 2 * h], p.scale_log2, fmaf(sl2, (float)(8 * nb), rb));
+                sv[4 * nb + 2 * h + 1] = fmaf(sv[4 * nb + 2 * h + 1], p.scale_log2, fmaf(sl2, (float)(8 * nb + 1), rb));
+              }
+            }
+          } else {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+              for (int c = 0; c < 32; ++c) {
+                const int j = tl * BN + 8 * (c >> 1) + 2 * (lane & 3) + (c & 1);
+                const int d = j < P ? j - cq[h] : (int)depth[(j - P) & 127] - dq[h];  // beyond the draft: hidden
+                const int r = 4 * (c >> 1) + 2 * h + (c & 1);
+                sv[r] = fmaf(sv[r], p.scale_log2, sl2 * (float)d);
+              }
+            }
+          }
+        }
         // row max: this thread's 32 columns, then the four lanes that share the row
         float m_new[2], m_use[2], alpha[2];
 #pragma unroll
@@ -542,7 +611,7 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
           float mx = fmaxf(mx0, mx1);
           mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 1));
           mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 2));
-          m_new[h] = fmaxf(m_run[h], mx * p.scale_log2);
+          m_new[h] = fmaxf(m_run[h], kAlibi ? mx : mx * p.scale_log2);  // ALiBi: already in the log2 domain
           m_use[h] = (m_new[h] == -INFINITY) ? 0.f : m_new[h];
           alpha[h] = (m_run[h] == -INFINITY) ? 0.f : ex2(m_run[h] - m_use[h]);
         }
@@ -554,8 +623,8 @@ k_tree_attn(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ C
 #pragma unroll
         for (int m = 0; m < 32; ++m) {  // ex2(-inf) = 0 for the hidden keys (m_use is finite)
           const int h = m & 1;
-          const float p0 = ex2(sv[2 * m] * p.scale_log2 - m_use[h]);
-          const float p1 = ex2(sv[2 * m + 1] * p.scale_log2 - m_use[h]);
+          const float p0 = ex2(kAlibi ? sv[2 * m] - m_use[h] : sv[2 * m] * p.scale_log2 - m_use[h]);
+          const float p1 = ex2(kAlibi ? sv[2 * m + 1] - m_use[h] : sv[2 * m + 1] * p.scale_log2 - m_use[h]);
           const __nv_bfloat162 b = __floats2bfloat162_rn(p0, p1);
           ls[h] += __bfloat162float(b.x) + __bfloat162float(b.y);
           pa[m] = *reinterpret_cast<const uint32_t *>(&b);
@@ -763,8 +832,10 @@ extern "C" int pia_attn_plan_create(const pia_attn_config_t *cfg, void *d_k_cach
   if (rc == PIA_OK) rc = encode_kv_map(&p->map_v, d_v_cache, *cfg);
   if (rc == PIA_OK) {
     cudaError_t e = cfg->head_dim == 64
-                        ? cudaFuncSetAttribute(k_tree_attn<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<64>::TOTAL)
-                        : cudaFuncSetAttribute(k_tree_attn<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<128>::TOTAL);
+                        ? cudaFuncSetAttribute(k_tree_attn<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<64>::TOTAL)
+                        : cudaFuncSetAttribute(k_tree_attn<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<128>::TOTAL);
+    if (e == cudaSuccess && cfg->head_dim == 128)
+      e = cudaFuncSetAttribute(k_tree_attn<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<128>::TOTAL);
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); rc = PIA_ERR_CUDA; }
   }
   p->dbg = nullptr;
@@ -792,9 +863,13 @@ extern "C" int pia_attn_plan_destroy(pia_attn_plan_t *p) {
 
 static int attn_launch(pia_attn_plan_t *p, int layer, const void *d_q, const void *d_qkv, const void *d_cos,
                        const void *d_sin, int max_pos, const uint64_t *d_mask, const pia_slots_t *slots, float scale_mul,
-                       void *d_out, void *stream) {
+                       void *d_out, void *stream, const float *d_slopes = nullptr) {
   const bool fused = d_qkv != nullptr;
   PIA_REQUIRE(p && (d_q || d_qkv) && d_mask && slots && slots->d_n && slots->d_prefix_len && d_out, "null argument");
+  if (d_slopes && p->cfg.head_dim != 128) {
+    set_error("head_dim %d: the ALiBi tree attention is built for head_dim 128 only", p->cfg.head_dim);
+    return PIA_ERR_UNSUPPORTED;
+  }
   PIA_REQUIRE(layer >= 0 && layer < p->cfg.n_layers, "layer %d outside [0,%d)", layer, p->cfg.n_layers);
   PIA_REQUIRE(slots->batch >= 1 && slots->batch <= 65535 && slots->rows_per_slot >= 1 &&
                   slots->rows_per_slot <= p->cfg.max_nodes, "bad slot table");
@@ -831,13 +906,17 @@ static int attn_launch(pia_attn_plan_t *p, int layer, const void *d_q, const voi
                               (long long)p->cfg.max_seq * p->cfg.head_dim;
   a.kc_layer = p->k_base + layer_off; a.vc_layer = p->v_base + layer_off;
   a.scale_log2 = scale_mul * 1.4426950408889634f / sqrtf((float)p->cfg.head_dim);
+  a.slopes = d_slopes;
   cudaStream_t s = (cudaStream_t)stream;
   const dim3 grid(ns, p->n_groups, slots->batch);
-  if (p->cfg.head_dim == 64)
-    PIA_CUDA_CHECK(launch_kernel_cluster(k_tree_attn<64>, grid, dim3(NTHREADS), Smem<64>::TOTAL, s, (unsigned)ns,
+  if (d_slopes)
+    PIA_CUDA_CHECK(launch_kernel_cluster(k_tree_attn<128, true>, grid, dim3(NTHREADS), Smem<128>::TOTAL, s,
+                                         (unsigned)ns, p->map_k, p->map_v, a));
+  else if (p->cfg.head_dim == 64)
+    PIA_CUDA_CHECK(launch_kernel_cluster(k_tree_attn<64, false>, grid, dim3(NTHREADS), Smem<64>::TOTAL, s, (unsigned)ns,
                                          p->map_k, p->map_v, a));
   else
-    PIA_CUDA_CHECK(launch_kernel_cluster(k_tree_attn<128>, grid, dim3(NTHREADS), Smem<128>::TOTAL, s, (unsigned)ns,
+    PIA_CUDA_CHECK(launch_kernel_cluster(k_tree_attn<128, false>, grid, dim3(NTHREADS), Smem<128>::TOTAL, s, (unsigned)ns,
                                          p->map_k, p->map_v, a));
   count_launch();
   return PIA_OK;
@@ -854,4 +933,11 @@ extern "C" int pia_tree_attn_fused_fwd(pia_attn_plan_t *p, int layer, const void
                                        float scale_mul, void *d_out, void *stream) {
   PIA_REQUIRE(d_qkv, "null qkv");
   return attn_launch(p, layer, nullptr, d_qkv, d_cos, d_sin, max_pos, d_mask, slots, scale_mul, d_out, stream);
+}
+
+extern "C" int pia_tree_attn_alibi_fwd(pia_attn_plan_t *p, int layer, const void *d_q, const uint64_t *d_mask,
+                                       const pia_slots_t *slots, float scale_mul, const float *d_slopes, void *d_out,
+                                       void *stream) {
+  PIA_REQUIRE(d_q && d_slopes, "null q / slopes");
+  return attn_launch(p, layer, d_q, nullptr, nullptr, nullptr, 0, d_mask, slots, scale_mul, d_out, stream, d_slopes);
 }
