@@ -321,6 +321,17 @@ int pia_silu_mul(const void *d_gate_up, int rows, int inter, void *d_out, void *
 /* embedding gather for the draft nodes: d_out[i] = table[d_ids[i]] (rows >= *d_n are zero filled) */
 int pia_embed_gather(const void *d_table, const int32_t *d_ids, const int32_t *d_n, int rows, int hidden, void *d_out,
                      void *stream);
+/* LayerNorm with weight and bias (BLOOM: bloom/modeling_bloom.py input_layernorm / post_attention_layernorm :346-349,
+ * word_embeddings_layernorm :422, ln_f :428).  If d_residual_in != NULL: x <- bf16(x + residual_in) first (dropout_add,
+ * :504 / :539); x is written to d_residual_out when that is not NULL.  Then y = bf16((x - mean) * rsqrt(var + eps) * w + b)
+ * with the biased variance, all arithmetic in fp32.  rows x hidden bf16; hidden % 8 == 0 and hidden <= 16384, else
+ * PIA_ERR_INVALID and nothing is launched.  y may alias x. */
+int pia_layernorm(const void *d_x, const void *d_residual_in, const void *d_weight, const void *d_bias, float eps,
+                  int rows, int hidden, void *d_residual_out, void *d_y, void *stream);
+/* BLOOM's tanh-GELU (bloom/modeling_bloom.py:194-203 bloom_gelu_forward): x * 0.5 * (1.0 + tanh(0.79788456 * x *
+ * (1 + 0.044715 * x * x))) over n bf16 elements, rounded to bf16 after every op as eager torch evaluates it (Python
+ * scalars in fp32).  n % 8 == 0, 16-byte aligned buffers; d_out may equal d_in (in place). */
+int pia_bloom_gelu(const void *d_in, int64_t n, void *d_out, void *stream);
 /* MoE combine (mixtral/modeling_mixtral.py:734-759, dense restatement): d_out[t] = sum_e d_expert_out[e][t] * w[t][e]
  * in expert-index order, product and partial sums rounded to bf16 as the eager bf16 loop does.
  * d_expert_out : [n_experts, rows_cap, hidden] bf16; d_weights : [rows, n_experts] bf16 routing weights (0 = expert not

@@ -100,6 +100,8 @@ SYMBOLS = {
                                          C.c_int, vp, vp, vp, C.c_int, vp]),
     'pia_silu_mul': (C.c_int, [vp, C.c_int, C.c_int, vp, vp]),
     'pia_embed_gather': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),
+    'pia_layernorm': (C.c_int, [vp, vp, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp]),
+    'pia_bloom_gelu': (C.c_int, [vp, C.c_int64, vp, vp]),
     'pia_moe_combine': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     'pia_moe_router': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     'pia_l2_prefetch': (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int64, C.c_float, vp]),

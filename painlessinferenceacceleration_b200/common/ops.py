@@ -31,6 +31,21 @@ def rmsnorm_partials(parts, residual_in, weight, eps, residual_out, y):
                                           rows, hidden, _p(residual_out), _p(y), _s()))
 
 
+def layernorm(x, residual_in, weight, bias, eps, residual_out, y):
+    """y = LayerNorm(x (+ residual_in)) with weight and bias; the residual sum goes to residual_out (pia_layernorm)"""
+    rows, hidden = x.shape
+    L.check(L.load().pia_layernorm(_p(x), _p(residual_in), _p(weight), _p(bias), float(eps), rows, hidden,
+                                   _p(residual_out), _p(y), _s()))
+
+
+def bloom_gelu(x, out=None):
+    """BLOOM's tanh-GELU with eager bf16 rounding (pia_bloom_gelu); out=None: in place"""
+    out = x if out is None else out
+    assert x.is_contiguous() and out.is_contiguous() and out.numel() == x.numel()
+    L.check(L.load().pia_bloom_gelu(_p(x), x.numel(), _p(out), _s()))
+    return out
+
+
 def tile_weight(w):
     """[N, K] -> [N/128, K/64, 128, 64] contiguous: one 16 KB block per (128-row tile, 64-wide k chunk), the unit the
     GEMM kernel's TMA box moves, so each CTA reads one contiguous slab of HBM"""

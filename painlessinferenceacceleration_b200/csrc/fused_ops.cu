@@ -6,6 +6,8 @@
 //                       with fp32 tables (baichuan2_7b/modeling_baichuan.py:148-155)
 //   k_silu_mul          :185-186
 //   k_embed_gather      :582
+//   k_layernorm         bloom/modeling_bloom.py LayerNorm with weight and bias (+ the residual add, dropout_add)
+//   k_bloom_gelu        bloom/modeling_bloom.py:194-203 bloom_gelu_forward
 // Rounding points follow the reference's bf16 eager arithmetic (each torch op rounds to bf16) so that
 // the verify logits stay as close to the reference's as a different GEMM order allows.
 #include <cuda_bf16.h>
@@ -223,6 +225,104 @@ __global__ void __launch_bounds__(256) k_embed_gather(const __nv_bfloat16 *table
   for (int v = threadIdx.x; v < nvec; v += 256) dst[v] = src[v];
 }
 
+// LayerNorm with weight and bias (bloom/modeling_bloom.py:346-349, :422, :428) over one row per CTA, preceded by the
+// residual add of the decoder block (dropout_add, :504 / :539: a bf16 add).  blockDim = min(512, nvec rounded up to a
+// warp); the row stays in registers (at most kLnVec 16-byte vectors per thread: hidden <= 512 * 8 * 4 = 16384) and the
+// mean and the biased variance are two fp32 passes over them.
+constexpr int kLnVec = 4;
+constexpr int kLnMaxHidden = 512 * 8 * kLnVec;
+
+__device__ __forceinline__ float block_sum(float v, float *red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float tot = 0.f;
+  const int nw = blockDim.x >> 5;
+  for (int i = 0; i < nw; ++i) tot += red[i];
+  return tot;
+}
+
+__global__ void __launch_bounds__(512) k_layernorm(const __nv_bfloat16 *x, const __nv_bfloat16 *res_in,
+                                                   const __nv_bfloat16 *w, const __nv_bfloat16 *b, float eps,
+                                                   int hidden, __nv_bfloat16 *res_out, __nv_bfloat16 *y) {
+  __shared__ float red[2][16];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int row = blockIdx.x, tid = threadIdx.x;
+  const int nvec = hidden >> 3;
+  const long long row_off = (long long)row * hidden;
+  const uint4 *xv = reinterpret_cast<const uint4 *>(x + row_off);
+  const uint4 *rv = res_in ? reinterpret_cast<const uint4 *>(res_in + row_off) : nullptr;
+  uint4 *rov = res_out ? reinterpret_cast<uint4 *>(res_out + row_off) : nullptr;
+  float f[kLnVec][8];
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < kLnVec; ++k) {
+    const int v = tid + k * blockDim.x;
+    if (v < nvec) {
+      Pack8 a; a.u = xv[v];
+      if (rv) {
+        Pack8 r; r.u = rv[v];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) a.h[j] = __float2bfloat16_rn(__bfloat162float(a.h[j]) + __bfloat162float(r.h[j]));
+      }
+      if (rov) rov[v] = a.u;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { f[k][j] = __bfloat162float(a.h[j]); s += f[k][j]; }
+    }
+  }
+  const float mean = block_sum(s, red[0]) / (float)hidden;
+  float ss = 0.f;
+#pragma unroll
+  for (int k = 0; k < kLnVec; ++k) {
+    if (tid + k * blockDim.x < nvec) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { const float d = f[k][j] - mean; ss += d * d; }
+    }
+  }
+  const float rstd = rsqrtf(block_sum(ss, red[1]) / (float)hidden + eps);
+  const uint4 *wv = reinterpret_cast<const uint4 *>(w);
+  const uint4 *bv = reinterpret_cast<const uint4 *>(b);
+  uint4 *yv = reinterpret_cast<uint4 *>(y + row_off);
+#pragma unroll
+  for (int k = 0; k < kLnVec; ++k) {
+    const int v = tid + k * blockDim.x;
+    if (v < nvec) {
+      Pack8 ww, bb, o;
+      ww.u = wv[v];
+      bb.u = bv[v];
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        o.h[j] = __float2bfloat16_rn((f[k][j] - mean) * rstd * __bfloat162float(ww.h[j]) + __bfloat162float(bb.h[j]));
+      yv[v] = o.u;
+    }
+  }
+}
+
+// BLOOM's tanh-GELU (bloom/modeling_bloom.py:194-203)
+//   x * 0.5 * (1.0 + tanh(0.79788456 * x * (1 + 0.044715 * x * x)))
+// evaluated as eager bf16 torch does: every op computes in fp32 with the Python scalars as fp32 and rounds to bf16.
+// Eight elements per thread; n % 8 == 0 and 16-byte aligned buffers.
+__device__ __forceinline__ float bloom_gelu1(float x) {
+  const float a = bf(x * 0.5f);
+  const float c = bf(bf(0.044715f * x) * x);
+  const float t = bf(bf(0.79788456f * x) * bf(c + 1.f));
+  return a * bf(bf(tanhf(t)) + 1.f);
+}
+
+__global__ void __launch_bounds__(256) k_bloom_gelu(const __nv_bfloat16 *in, long long nvec, __nv_bfloat16 *out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += (long long)gridDim.x * blockDim.x) {
+    Pack8 a, o;
+    a.u = reinterpret_cast<const uint4 *>(in)[v];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o.h[j] = __float2bfloat16_rn(bloom_gelu1(__bfloat162float(a.h[j])));
+    reinterpret_cast<uint4 *>(out)[v] = o.u;
+  }
+}
+
 }  // namespace fused
 }  // namespace pia
 
@@ -302,6 +402,31 @@ extern "C" int pia_silu_mul(const void *d_gate_up, int rows, int inter, void *d_
   dim3 grid((inter / 8 + 255) / 256, rows);
   PIA_CUDA_CHECK(launch_kernel(k_silu_mul, grid, dim3(256), 0, (cudaStream_t)stream, (const __nv_bfloat16 *)d_gate_up,
                               inter, (__nv_bfloat16 *)d_out));
+  count_launch();
+  return PIA_OK;
+}
+
+extern "C" int pia_layernorm(const void *d_x, const void *d_residual_in, const void *d_weight, const void *d_bias,
+                             float eps, int rows, int hidden, void *d_residual_out, void *d_y, void *stream) {
+  PIA_REQUIRE(d_x && d_weight && d_bias && d_y && rows > 0 && hidden > 0 && hidden % 8 == 0 && hidden <= kLnMaxHidden,
+              "bad layernorm arguments: hidden must be a positive multiple of 8, at most 16384");
+  const int nvec = hidden / 8;
+  const int threads = nvec >= 512 ? 512 : (nvec + 31) / 32 * 32;
+  PIA_CUDA_CHECK(launch_kernel(k_layernorm, dim3(rows), dim3(threads), 0, (cudaStream_t)stream,
+                              (const __nv_bfloat16 *)d_x, (const __nv_bfloat16 *)d_residual_in,
+                              (const __nv_bfloat16 *)d_weight, (const __nv_bfloat16 *)d_bias, eps, hidden,
+                              (__nv_bfloat16 *)d_residual_out, (__nv_bfloat16 *)d_y));
+  count_launch();
+  return PIA_OK;
+}
+
+extern "C" int pia_bloom_gelu(const void *d_in, int64_t n, void *d_out, void *stream) {
+  PIA_REQUIRE(d_in && d_out && n > 0 && n % 8 == 0 && ((uintptr_t)d_in & 15) == 0 && ((uintptr_t)d_out & 15) == 0,
+              "bad bloom_gelu arguments: n must be a positive multiple of 8, buffers 16-byte aligned");
+  const long long nvec = n / 8;
+  const long long blocks = (nvec + 255) / 256;
+  PIA_CUDA_CHECK(launch_kernel(k_bloom_gelu, dim3((unsigned)(blocks < 65536 ? blocks : 65536)), dim3(256), 0,
+                              (cudaStream_t)stream, (const __nv_bfloat16 *)d_in, nvec, (__nv_bfloat16 *)d_out));
   count_launch();
   return PIA_OK;
 }
