@@ -5,13 +5,13 @@ fp32-RoPE verify forward (every draft node's logits = a causal forward over pref
 models (tests/tiny_baichuan.py) through generate(), the oracle loop, checkpoint loading and fp8.  `big`: the
 Baichuan-13B and Baichuan2-7B shapes through the loop."""
 import json
-import math
 
 import numpy as np
 import pytest
 import torch
 from torch.nn import functional as F
 
+from tests import attn_ref
 from tests.test_gpu_fp8 import _same_bytes
 from tests.test_gpu_generate import OursBackend
 from tests.test_gpu_head_dim64 import _mask, _tree
@@ -29,26 +29,10 @@ D = 128
 # the kernel: pia_tree_attn_alibi_fwd
 # ---------------------------------------------------------------------------------------------------------------
 def _ref_alibi(q, kc, vc, rows, n, P, pad, G, slopes):
-    """fp32 restatement: row i (tree depth t_i = popc(rows[i]) - 1) at qpos = max(P - pad, 0) + t_i; cached key j in
-    [pad, P) at kpos = j - pad, draft key k (an ancestor of i, or i) at max(P - pad, 0) + t_k; score = q.k / sqrt(D) +
-    slope_h * (kpos - qpos); softmax in fp32"""
-    base = max(P - pad, 0)
-    depth = torch.tensor([bin(r).count('1') - 1 for r in rows], dtype=torch.float32, device=DEV)
-    qpos = base + depth                                                          # [n]
-    kpos = torch.cat([torch.arange(P, device=DEV, dtype=torch.float32) - pad, base + depth])   # [P + n]
-    vis = torch.zeros((n, P + n), dtype=torch.bool, device=DEV)
-    vis[:, pad:P] = True
-    for i, r in enumerate(rows):
-        for j in range(n):
-            if (r >> j) & 1:
-                vis[i, P + j] = True
-    Hq = q.shape[1]
-    k = kc[:, :P + n].float().repeat_interleave(G, 0)      # [Hq, P + n, D]
-    v = vc[:, :P + n].float().repeat_interleave(G, 0)
-    s = torch.einsum('ihd,hjd->hij', q[:n].float(), k) / math.sqrt(D)
-    s = s + slopes[:, None, None] * (kpos[None, None, :] - qpos[None, :, None])
-    s = s.masked_fill(~vis[None], float('-inf'))
-    return torch.einsum('hij,hjd->ihd', torch.softmax(s, -1), v)
+    """exact (fp64) restatement: row i (tree depth t_i = popc(rows[i]) - 1) at qpos = max(P - pad, 0) + t_i; cached
+    key j in [pad, P) at kpos = j - pad, draft key k (an ancestor of i, or i) at max(P - pad, 0) + t_k; score =
+    q.k / sqrt(D) + slope_h * (kpos - qpos) (tests/attn_ref.py)"""
+    return attn_ref.reference(q, kc, vc, rows, n, P, pad, G, slopes=slopes)
 
 
 def _slopes(H):
@@ -85,7 +69,7 @@ def test_alibi_tree_attention(Hq, Hkv, P, n, R):
         torch.cuda.synchronize()
         ref = _ref_alibi(q, kc[layer], vc[layer], rows, n, P, pad, Hq // Hkv, slopes)
         err = (out[:n].float() - ref).abs().max().item()
-        assert torch.allclose(out[:n].float(), ref, atol=1.5e-2, rtol=2e-2), f'layer {layer} max abs err {err}'
+        attn_ref.assert_close(out[:n].float(), ref, f'layer {layer} max abs err {err}')
         assert float((out[n:].float() - 9.0).abs().sum()) == 0
 
 
@@ -109,7 +93,7 @@ def test_alibi_bias_is_not_a_no_op():
     assert (a[:n, 0].float() - b[:n, 0].float()).abs().max().item() > 0.3
     assert torch.equal(a[:n, 3], b[:n, 3])   # slope 0: the plain arithmetic
     ref = _ref_alibi(q, kc[0], vc[0], rows, n, P, 0, 1, slopes)
-    assert torch.allclose(a[:n].float(), ref, atol=1.5e-2, rtol=2e-2)
+    attn_ref.assert_close(a[:n].float(), ref)
 
 
 @pytest.mark.parametrize('R,rps', [(64, 16), (128, 32)])
@@ -138,7 +122,7 @@ def test_alibi_several_slots(R, rps):
         assert float((out[r0 + n:r0 + rps].float() - 9.0).abs().sum()) == 0
         if n:
             ref = _ref_alibi(q[r0:], kc[s_, 0], vc[s_, 0], rows, n, P, pad, Hq // Hkv, slopes)
-            assert torch.allclose(out[r0:r0 + n].float(), ref, atol=1.5e-2, rtol=2e-2), s_
+            attn_ref.assert_close(out[r0:r0 + n].float(), ref, s_)
 
 
 def test_alibi_head_dim64_is_unsupported():

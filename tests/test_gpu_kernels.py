@@ -1,11 +1,12 @@
 # -*- coding: utf-8 -*-
 """Numerics of the verify-forward kernels against plain PyTorch fp32 restatements of the reference ops
 (models/llama/modeling_llama.py:76-90, 156-169, 185-186, 243-308; pretrained_model.py:764-892, 894-907)."""
-import math
 
 import numpy as np
 import pytest
 import torch
+
+from tests import attn_ref
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -46,25 +47,8 @@ def _slots(ns, Ps, pads, rows_per_slot, stride=0, first=0):
 
 
 def _ref_attention(q, kc, vc, rows, n, P, pad_len, G):
-    """eager attention of the reference with the [n, P+n] lookahead mask; fp32 scores, probabilities rounded to
-    bf16 before PV exactly like modeling_llama.py:291-292"""
-    Hq, D = q.shape[1], q.shape[2]
-    L = P + n
-    vis = torch.zeros((n, L), dtype=torch.bool, device=q.device)
-    vis[:, pad_len:P] = True
-    for i in range(n):
-        for j in range(n):
-            if (int(rows[i]) >> j) & 1:
-                vis[i, P + j] = True
-    out = torch.zeros((n, Hq, D), dtype=torch.float32, device=q.device)
-    for h in range(Hq):
-        k = kc[h // G, :L].float()
-        v = vc[h // G, :L].float()
-        s = (q[:n, h].float() @ k.t()) / math.sqrt(D)
-        s = s.masked_fill(~vis, float('-inf'))
-        p = torch.softmax(s, dim=-1).to(torch.bfloat16).float()
-        out[:, h] = p @ v
-    return out
+    """eager attention of the reference with the [n, P+n] lookahead mask, exact (fp64; tests/attn_ref.py)"""
+    return attn_ref.reference(q, kc, vc, rows, n, P, pad_len, G)
 
 
 @pytest.mark.parametrize('Hq,Hkv,P,n,pad', [(2, 2, 0, 64, 0), (4, 2, 37, 33, 0), (32, 32, 300, 64, 0),
@@ -93,7 +77,7 @@ def test_tree_attention(Hq, Hkv, P, n, pad):
         got = out[:n].float()
         err = (got - ref).abs().max().item()
         # tolerance: bf16 output rounding (2^-8 relative on |o| <~ 1) + fp32 accumulation order
-        assert torch.allclose(got, ref, atol=1.5e-2, rtol=2e-2), f'layer {layer} max abs err {err}'
+        attn_ref.assert_close(got, ref, f'layer {layer} max abs err {err}')
 
 
 def test_rmsnorm_residual():
@@ -306,7 +290,7 @@ def test_batched_slots_rope_and_attention(Hq, Hkv, rps, cases):
         assert float((ob[r0 + n:r0 + rps].float() - 9.0).abs().sum()) == 0
         if n:
             ref = _ref_attention(q1, kc[s_, layer], vc[s_, layer], trees[s_], n, P, pad, Hq // Hkv)
-            assert torch.allclose(ob[r0:r0 + n].float(), ref, atol=1.5e-2, rtol=2e-2)
+            attn_ref.assert_close(ob[r0:r0 + n].float(), ref)
 
 
 @pytest.mark.parametrize('Hq,Hkv,rps,cases', [
@@ -356,7 +340,7 @@ def test_fused_rope_kv_append_attention(Hq, Hkv, rps, cases):
         assert torch.allclose(o2[r0:r0 + n].float(), o1[r0:r0 + n].float(), atol=4e-3, rtol=2e-2), s_
         assert float((o2[r0 + n:r0 + rps].float() - 9.0).abs().sum()) == 0      # rows beyond the draft: untouched
         ref = _ref_attention(q[r0:], kc[s_, layer], vc[s_, layer], trees[s_], n, P, pad, Hq // Hkv)
-        assert torch.allclose(o2[r0:r0 + n].float(), ref, atol=1.5e-2, rtol=2e-2), s_
+        attn_ref.assert_close(o2[r0:r0 + n].float(), ref, s_)
 
 
 def test_prefill_chunks_share_one_cache():
