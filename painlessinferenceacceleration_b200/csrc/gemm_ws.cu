@@ -346,8 +346,9 @@ struct SkParams {
   int *flags;           // [n_tiles], zero between launches
 };
 
-__device__ __forceinline__ long long sk_begin(long long b, long long U, int G) { return b * U / G; }
-__device__ __forceinline__ int sk_cta_of(long long x, long long U, int G) {
+// shared with the host, which sizes the fix-up workspace from the same partition
+__host__ __device__ __forceinline__ long long sk_begin(long long b, long long U, int G) { return b * U / G; }
+__host__ __device__ __forceinline__ int sk_cta_of(long long x, long long U, int G) {
   int b = (int)(x * G / U);
   while (b + 1 < G && sk_begin(b + 1, U, G) <= x) ++b;
   while (b > 0 && sk_begin(b, U, G) > x) --b;
@@ -839,8 +840,14 @@ extern "C" int pia_gemm_plan_create(const void *d_w, int N, int K, const void *d
     k.N = N; k.n_tiles = N / BMW; k.n_chunks = n_chunks; k.rows = TOK;
     k.units = (long long)k.n_tiles * n_chunks;
     g->sk_grid = (int)(k.units < n_sm ? k.units : n_sm);
-    const long long per = (k.units + g->sk_grid - 1) / g->sk_grid;
-    k.max_contrib = (int)((n_chunks + per - 1) / per) + 1;
+    // contributor slots of a tile = the CTAs after its owner that hold some of its chunks.  The ranges are
+    // floor(U/G) or ceil(U/G) units long, so the count is read off the partition itself, tile by tile.
+    k.max_contrib = 1;
+    for (int t = 0; t < k.n_tiles; ++t) {
+      const long long ts = (long long)t * n_chunks;
+      const int c = sk_cta_of(ts + n_chunks - 1, k.units, g->sk_grid) - sk_cta_of(ts, k.units, g->sk_grid);
+      if (c > k.max_contrib) k.max_contrib = c;
+    }
     k.out = nullptr;
     cudaError_t e = cudaMalloc((void **)&k.ws, sizeof(float) * (size_t)k.n_tiles * k.max_contrib * BMW * TOK);
     if (e == cudaSuccess) e = cudaMalloc((void **)&k.flags, sizeof(int) * k.n_tiles);

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import gemm_ref
 from tests.test_gpu_generate import EPS, OursBackend
 from tests.tiny_models import prompts, tiny_hf_model
 from tests.tiny_qwen2 import qwen2_hf_model
@@ -66,17 +67,15 @@ ROWS = (1, 5, 64, 128, 256)
 
 @pytest.mark.parametrize('name,N,K,biased,splits', SHAPES)
 def test_fp8_gemm_against_fp32(name, N, K, biased, splits):
-    """out = bf16(X @ deq(W)^T (+ bias)) within one bf16 rounding of the fp32 result for 1..256 rows and every split
-    mode (plain, cluster split-K, fp32 slices); two runs bit-identical; rows beyond `rows` untouched"""
+    """out = bf16(X @ deq(W)^T (+ bias)) against the fp64 reference with the comparator of tests/gemm_ref.py, for
+    1..256 rows and every split mode (plain, cluster split-K, fp32 slices); two runs bit-identical; rows beyond `rows`
+    untouched"""
     ops = _ops()
     q, s = _quantised((N, K), seed=N + K)
-    deq = q.float() * s[:, None]
     qw = ops.tile_weight_fp8(q)
     x = torch.randn((256, K), generator=torch.Generator(device=DEV).manual_seed(1), device=DEV).to(torch.bfloat16)
     bias = (torch.randn(N, device=DEV) * 2).to(torch.bfloat16).float() if biased else None
-    ref = x.float() @ deq.t()
-    if bias is not None:
-        ref = ref + bias
+    ref, mass = gemm_ref.reference(x, q, s, bias)
     for sk in splits:
         g = ops.Gemm.fp8(qw, s, x, bias=bias, split_k=sk)
         for rows in ROWS:
@@ -93,7 +92,8 @@ def test_fp8_gemm_against_fp32(name, N, K, biased, splits):
             else:
                 assert (o1[rows:] == 7.0).all(), (name, sk, rows)
                 got = o1[:rows]
-            torch.testing.assert_close(got.float(), ref[:rows], atol=2e-2, rtol=1.6e-2, msg=f'{name} split {sk} rows {rows}')
+            gemm_ref.assert_close(got, ref[:rows], mass[:rows], K, g.splits if sk > 0 else -sk,
+                                  f'{name} split {sk} rows {rows}')
 
 
 def test_fp8_mixtral_stacked_gate_up_and_grouped_down():
@@ -105,8 +105,8 @@ def test_fp8_mixtral_stacked_gate_up_and_grouped_down():
     x = torch.randn((256, H), generator=torch.Generator(device=DEV).manual_seed(2), device=DEV).to(torch.bfloat16)
     g = ops.Gemm.fp8(ops.tile_weight_fp8(q), s, x)
     for rows in (1, 64, 256):
-        ref = x[:rows].float() @ (q.float() * s[:, None]).t()
-        torch.testing.assert_close(g.run(rows)[:rows].float(), ref, atol=2e-2, rtol=1.6e-2)
+        ref, mass = gemm_ref.reference(x[:rows], q, s)
+        gemm_ref.assert_close(g.run(rows)[:rows], ref, mass, H, 1, f'gate_up rows {rows}')
     del g, q, s
     q, s = _quantised((E, H, I), seed=4)
     xa = torch.randn((256, E * I), generator=torch.Generator(device=DEV).manual_seed(3), device=DEV).to(torch.bfloat16)
@@ -116,8 +116,8 @@ def test_fp8_mixtral_stacked_gate_up_and_grouped_down():
         out = g.run(rows)
         assert (out[:, rows:] == 7.0).all()
         for e in (0, 5, 7):
-            ref = xa[:rows, e * I:(e + 1) * I].float() @ (q[e].float() * s[e][:, None]).t()
-            torch.testing.assert_close(out[e, :rows].float(), ref, atol=2e-2, rtol=1.6e-2)
+            ref, mass = gemm_ref.reference(xa[:rows, e * I:(e + 1) * I], q[e], s[e])
+            gemm_ref.assert_close(out[e, :rows], ref, mass, I, 1, f'expert {e} rows {rows}')
 
 
 @pytest.mark.parametrize('rows', [5, 64, 200])
