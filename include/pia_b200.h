@@ -367,6 +367,10 @@ typedef struct {
   int32_t bound_walk;          /* 1: the walk accepts at most max_length - seq_len tokens, the batched loop's
                                   range(-1, min(max_branch_length, max_length - cur - 2)) (pretrained_model_batch.py:862);
                                   0: unbounded (the per-request loop clamps the draft depth instead, :680) */
+  float inv_repetition_penalty; /* (float)(1.0 / p) with p the caller's double: a positive score s is penalised to
+                                   bf16(s * inv_repetition_penalty), as PyTorch's CUDA division by a Python scalar
+                                   computes s / p; a negative one to bf16(s * repetition_penalty).  Must be
+                                   set: pia_accept refuses a value <= 0 (e.g. a zeroed field)             */
 } pia_accept_config_t;
 
 /* Row arg-max of the (penalised) logits of every draft node, then the walk of :827-860 (batched loop:

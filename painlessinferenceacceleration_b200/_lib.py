@@ -38,7 +38,8 @@ class AttnConfig(C.Structure):
 
 class AcceptConfig(C.Structure):
     _fields_ = [('vocab', C.c_int32), ('max_nodes', C.c_int32), ('repetition_penalty', C.c_float),
-                ('n_eos', C.c_int32), ('eos', C.c_int32 * 8), ('max_length', C.c_int32), ('bound_walk', C.c_int32)]
+                ('n_eos', C.c_int32), ('eos', C.c_int32 * 8), ('max_length', C.c_int32), ('bound_walk', C.c_int32),
+                ('inv_repetition_penalty', C.c_float)]
 
 
 class Slots(C.Structure):

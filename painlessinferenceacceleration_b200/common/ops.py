@@ -372,8 +372,11 @@ class Accept(object):
     def __init__(self, vocab, max_nodes, repetition_penalty, eos_ids, max_length, device, bound_walk=False):
         eos = [int(e) for e in (eos_ids or []) if e is not None][:8]
         arr = (C.c_int32 * 8)(*(eos + [-1] * (8 - len(eos))))
+        # the reciprocal in double, rounded once to fp32: what RepetitionPenaltyLogitsProcessor's score / penalty
+        # multiplies by on CUDA
         self.cfg = L.AcceptConfig(vocab, max_nodes, float(repetition_penalty), len(eos), arr, int(max_length),
-                                  int(bool(bound_walk)))
+                                  int(bool(bound_walk)),
+                                  1.0 / float(repetition_penalty) if repetition_penalty > 0 else 0.0)
         self.max_nodes = max_nodes
         self.lib = L.load()
         self.workspace = torch.empty((max(self.lib.pia_accept_workspace_bytes(C.byref(self.cfg)) // 4, 1),),

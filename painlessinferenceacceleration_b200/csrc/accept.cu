@@ -32,13 +32,20 @@ __device__ __forceinline__ float gumbel(unsigned seed, unsigned counter, unsigne
 
 constexpr int NT = 1024;
 
+// (v, i) comes first in torch.argmax order: a NaN above every number, then the larger value, then the lower index
+__device__ __forceinline__ bool beats(float v, int i, float best, int best_i) {
+  const bool vn = v != v, bn = best != best;
+  if (vn != bn) return vn;
+  return v > best || ((vn || v == best) && i < best_i);
+}
+
 // grid = batch * rows_per_slot activation rows (rows >= n of their slot idle).  dynamic smem: vocab bits (only when
 // penalty != 1)
 __global__ void __launch_bounds__(NT) k_row_argmax(const __nv_bfloat16 *logits, int vocab, const int *ids,
                                                    const unsigned long long *mask, int mask_words, const int *d_n,
                                                    int rows_per_slot, const int *seq, int seq_stride,
-                                                   const int *d_seq_len, float penalty, const unsigned *rng,
-                                                   int *row_tok) {
+                                                   const int *d_seq_len, float penalty, float inv_penalty,
+                                                   const unsigned *rng, int *row_tok) {
   extern __shared__ unsigned bits[];
   __shared__ float s_val[NT / 32];
   __shared__ int s_idx[NT / 32];
@@ -81,9 +88,13 @@ __global__ void __launch_bounds__(NT) k_row_argmax(const __nv_bfloat16 *logits, 
       const int t = v0 + j;
       if (t >= vocab) break;
       float x = __bfloat162float(h[j]);
-      if (pen && ((bits[t >> 5] >> (t & 31)) & 1u)) x = x < 0.f ? bf(x * penalty) : bf(x / penalty);
+      // RepetitionPenaltyLogitsProcessor: score * p below zero, else score / p - which PyTorch's CUDA true division
+      // by a Python scalar computes as score * fl32(1 / p), the reciprocal taken in double (div_true_kernel_cuda)
+      if (pen && ((bits[t >> 5] >> (t & 31)) & 1u)) x = x < 0.f ? bf(x * penalty) : bf(x * inv_penalty);
       if (sample) x += gumbel(seed, counter, (unsigned)row, (unsigned)t);
-      if (x > best) { best = x; best_i = t; }  // ascending t inside a thread keeps the first maximum
+      // torch.argmax order: !(x <= best) also takes a NaN, and once best is a NaN nothing replaces it; ascending t
+      // inside a thread keeps the first maximum
+      if (!(x <= best) && best == best) { best = x; best_i = t; }
     }
   }
   // first-index arg-max (torch.argmax returns the first maximal index)
@@ -91,7 +102,7 @@ __global__ void __launch_bounds__(NT) k_row_argmax(const __nv_bfloat16 *logits, 
   for (int o = 16; o > 0; o >>= 1) {
     const float ov = __shfl_xor_sync(FULL, best, o);
     const int oi = __shfl_xor_sync(FULL, best_i, o);
-    if (ov > best || (ov == best && oi < best_i)) { best = ov; best_i = oi; }
+    if (beats(ov, oi, best, best_i)) { best = ov; best_i = oi; }
   }
   if ((tid & 31) == 0) { s_val[tid >> 5] = best; s_idx[tid >> 5] = best_i; }
   __syncthreads();
@@ -101,7 +112,7 @@ __global__ void __launch_bounds__(NT) k_row_argmax(const __nv_bfloat16 *logits, 
     for (int o = 16; o > 0; o >>= 1) {
       const float ov = __shfl_xor_sync(FULL, best, o);
       const int oi = __shfl_xor_sync(FULL, best_i, o);
-      if (ov > best || (ov == best && oi < best_i)) { best = ov; best_i = oi; }
+      if (beats(ov, oi, best, best_i)) { best = ov; best_i = oi; }
     }
     if (tid == 0) row_tok[row] = best_i == 0x7fffffff ? 0 : best_i;
   }
@@ -212,7 +223,8 @@ extern "C" int pia_accept(const pia_accept_config_t *cfg, const void *d_logits, 
   PIA_REQUIRE(batch >= 1 && rows_per_slot >= 1 && batch * rows_per_slot <= cfg->max_nodes,
               "batch * rows_per_slot must fit the %d draft rows", cfg->max_nodes);
   PIA_REQUIRE(cfg->vocab > 0 && cfg->n_eos >= 0 && cfg->n_eos <= 8, "bad accept config");
-  PIA_REQUIRE(cfg->repetition_penalty > 0.f, "repetition_penalty must be > 0");
+  PIA_REQUIRE(cfg->repetition_penalty > 0.f && cfg->inv_repetition_penalty > 0.f,
+              "repetition_penalty and its reciprocal must be > 0");
   cudaStream_t s = (cudaStream_t)stream;
   int *row_tok = (int *)d_workspace;
   const bool pen = cfg->repetition_penalty != 1.0f;
@@ -225,7 +237,8 @@ extern "C" int pia_accept(const pia_accept_config_t *cfg, const void *d_logits, 
   k_row_argmax<<<batch * rows_per_slot, accept::NT, smem, s>>>((const __nv_bfloat16 *)d_logits, cfg->vocab, d_ids,
                                                               (const unsigned long long *)d_mask, mask_words, d_n,
                                                               rows_per_slot, d_seq, seq_stride, d_seq_len,
-                                                              cfg->repetition_penalty, d_rng, row_tok);
+                                                              cfg->repetition_penalty, cfg->inv_repetition_penalty,
+                                                              d_rng, row_tok);
   PIA_LAUNCH_CHECK();
   k_accept_walk<<<batch, 128, 0, s>>>(*cfg, row_tok, d_ids, (const unsigned long long *)d_mask, mask_words, d_n,
                                       rows_per_slot, d_seq, seq_stride, d_seq_len, d_max_length, d_rng, d_accept_tokens,
