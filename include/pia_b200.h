@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define PIA_ABI_VERSION 2
+#define PIA_ABI_VERSION 3
 
 typedef enum {
   PIA_OK = 0,
@@ -283,15 +283,24 @@ int pia_gemm_plan_create_grouped_fp8(const void *d_w, const void *d_scale, int g
 /* ============================================================================================
  * Fused elementwise pieces of the verify forward (all bf16 I/O, fp32 math)
  * ============================================================================================ */
-/* RMSNorm (modeling_llama.py:76-90): y = (w * (x * rsqrt(mean(x^2)+eps)).to(bf16)) ; rows x hidden.
- * If d_residual_in != NULL: x <- x + residual_in first and the sum is written to d_residual_out. */
-int pia_rmsnorm(const void *d_x, const void *d_residual_in, const void *d_weight, float eps, int rows, int hidden,
-                void *d_residual_out, void *d_y, void *stream);
+/* RMSNorm (modeling_llama.py:76-90) over rows x hidden; hidden a positive multiple of 8, at most 16384, else
+ * PIA_ERR_INVALID and nothing is launched.  If d_residual_in != NULL: x <- bf16(x + residual_in) first, and that sum
+ * is written to d_residual_out when it is not NULL (d_residual_out may be d_residual_in: the in-place update of the
+ * decoder layer).  x_hat = x * rsqrt(mean(x^2) + eps) in fp32, then by `rounding`:
+ *   PIA_RMSNORM_ROUND_ONCE:  y = bf16(w * x_hat)        (llama/modeling_llama.py:90, chatglm/modeling_chatglm.py:187)
+ *   PIA_RMSNORM_ROUND_TWICE: y = bf16(w * bf16(x_hat))  (mistral/modeling_mistral.py:90, mixtral/modeling_mixtral.py:165,
+ *                            qwen2/modeling_qwen2.py:96, baichuan_7b/modeling_baichuan.py:84-91 and the other
+ *                            Baichuan members, transformers' GlmRMSNorm / Glm4RMSNorm)
+ * any other value: PIA_ERR_INVALID. */
+enum { PIA_RMSNORM_ROUND_ONCE = 0, PIA_RMSNORM_ROUND_TWICE = 1 };
+int pia_rmsnorm(const void *d_x, const void *d_residual_in, const void *d_weight, float eps, int rounding, int rows,
+                int hidden, void *d_residual_out, void *d_y, void *stream);
 /* same, with x given as `n_parts` fp32 split-K slices of pia_gemm_run ([n_parts][part_stride] floats, row-major
- * [rows, hidden] inside a slice): x = bf16(sum of slices), i.e. what a bf16 GEMM output would have held */
+ * [rows, hidden] inside a slice): x = bf16(((p0 + p1) + p2) + ...) summed in fp32 in slice order, i.e. what a bf16 GEMM
+ * output would have held */
 int pia_rmsnorm_partials(const float *d_x_parts, int n_parts, int64_t part_stride, const void *d_residual_in,
-                         const void *d_weight, float eps, int rows, int hidden, void *d_residual_out, void *d_y,
-                         void *stream);
+                         const void *d_weight, float eps, int rounding, int rows, int hidden, void *d_residual_out,
+                         void *d_y, void *stream);
 /* RoPE at tree positions + KV append (modeling_llama.py:261-268, 93-169; batched: modeling_llama_batch.py:375-405;
  * position of node i of slot s = max(P_s - pad_s, 0) + depth_i = rowsum(mask) - 1, :587).
  * d_qkv : [batch * rows_per_slot, (Hq + 2*Hkv) * D] bf16 (fused projection output).  d_cos / d_sin : [max_pos, D/2]

@@ -17,6 +17,7 @@ MODE = {'input': 0, 'output': 1, 'mix': 2}
 GET_HIER, GET_ONE = 0, 1
 GET_TAIL = 1
 GET_FIRST_ONLY = 2
+RMSNORM_ROUND_ONCE, RMSNORM_ROUND_TWICE = 0, 1   # pia_rmsnorm's `rounding`
 
 
 class TrieConfig(C.Structure):
@@ -82,8 +83,9 @@ SYMBOLS = {
     'pia_tree_attn_fwd': (C.c_int, [vp, C.c_int, vp, vp, C.POINTER(Slots), C.c_float, vp, vp]),
     'pia_tree_attn_fused_fwd': (C.c_int, [vp, C.c_int, vp, vp, vp, C.c_int, vp, C.POINTER(Slots), C.c_float, vp, vp]),
     'pia_tree_attn_alibi_fwd': (C.c_int, [vp, C.c_int, vp, vp, C.POINTER(Slots), C.c_float, vp, vp, vp]),
-    'pia_rmsnorm': (C.c_int, [vp, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp]),
-    'pia_rmsnorm_partials': (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp]),
+    'pia_rmsnorm': (C.c_int, [vp, vp, vp, C.c_float, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
+    'pia_rmsnorm_partials': (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, C.c_float, C.c_int, C.c_int, C.c_int, vp, vp,
+                                       vp]),
     'pia_gemm_plan_create': (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
     'pia_gemm_plan_create_grouped': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.POINTER(vp)]),
     'pia_gemm_plan_create_fp8': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.POINTER(vp)]),

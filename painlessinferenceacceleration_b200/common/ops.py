@@ -17,18 +17,23 @@ def _p(t):
     return t.data_ptr() if t is not None else None
 
 
-def rmsnorm(x, residual_in, weight, eps, residual_out, y):
+ROUND_ONCE, ROUND_TWICE = L.RMSNORM_ROUND_ONCE, L.RMSNORM_ROUND_TWICE
+
+
+def rmsnorm(x, residual_in, weight, eps, residual_out, y, *, rounding=ROUND_ONCE):
+    """y = RMSNorm(x (+ residual_in)), the residual sum to residual_out (pia_rmsnorm).  rounding: ROUND_ONCE,
+    bf16(w * x_hat) (Llama, ChatGLM), or ROUND_TWICE, bf16(w * bf16(x_hat)) (Mistral, Mixtral, Qwen2, Baichuan, GLM)"""
     rows, hidden = x.shape
-    L.check(L.load().pia_rmsnorm(_p(x), _p(residual_in), _p(weight), float(eps), rows, hidden, _p(residual_out),
-                                 _p(y), _s()))
+    L.check(L.load().pia_rmsnorm(_p(x), _p(residual_in), _p(weight), float(eps), int(rounding), rows, hidden,
+                                 _p(residual_out), _p(y), _s()))
 
 
-def rmsnorm_partials(parts, residual_in, weight, eps, residual_out, y):
-    """parts: fp32 [n_parts, 64, hidden] split-K slices of a Gemm"""
+def rmsnorm_partials(parts, residual_in, weight, eps, residual_out, y, *, rounding=ROUND_ONCE):
+    """parts: fp32 [n_parts, 64, hidden] split-K slices of a Gemm; rounding as rmsnorm"""
     n_parts, prow, hidden = parts.shape
     rows = y.shape[0]
     L.check(L.load().pia_rmsnorm_partials(_p(parts), n_parts, prow * hidden, _p(residual_in), _p(weight), float(eps),
-                                          rows, hidden, _p(residual_out), _p(y), _s()))
+                                          int(rounding), rows, hidden, _p(residual_out), _p(y), _s()))
 
 
 def layernorm(x, residual_in, weight, bias, eps, residual_out, y):

@@ -1,5 +1,6 @@
 // Elementwise pieces of the LOOKAHEAD verify forward (sm_90a), all HBM-bound, 16-byte vectorised:
-//   k_rmsnorm           models/llama/modeling_llama.py:76-90   (+ the residual add of the decoder layer :340-352)
+//   k_rmsnorm           models/llama/modeling_llama.py:76-90   (+ the residual add of the decoder layer :340-352), in
+//                       the rounding of the family's own norm (one or two bf16 roundings, see k_rmsnorm)
 //   k_rope_kv_append    :156-169 apply_rotary_pos_emb at the tree positions of :587, and the KV-cache append
 //                       that replaces the reference's per-step torch.cat (:265-268); a second instance rotates in
 //                       the GLM layout (chatglm/modeling_chatglm.py:156-169, positions :815), a third one in fp32
@@ -40,6 +41,17 @@ __device__ __forceinline__ Pack8 load_x8(const __nv_bfloat16 *x, const float *pa
   return a;
 }
 
+// the whole row stays in registers: at most kRmsVec 16-byte vectors per thread, hidden <= 512 * 8 * kRmsVec = 16384.
+// Thread t owns vectors t, t + 512, ...; its squares are summed serially in that order, then over the warp (5 shuffle
+// levels) and over the 16 warps (serially, warp order).
+// kRoundTwice selects where the normalised value x_hat = x * rsqrt(mean(x^2) + eps) is rounded:
+//   false: y = bf16(w * x_hat)        (llama/modeling_llama.py:90, chatglm/modeling_chatglm.py:187)
+//   true:  y = bf16(w * bf16(x_hat))  (mistral/modeling_mistral.py:90, qwen2/modeling_qwen2.py:96, Baichuan, GLM HF)
+// The product of two bf16 values is exact in fp32, so the second form has one more rounding and no other difference.
+constexpr int kRmsVec = 4;
+constexpr int kRmsMaxHidden = 512 * 8 * kRmsVec;
+
+template <bool kRoundTwice>
 __global__ void __launch_bounds__(512) k_rmsnorm(const __nv_bfloat16 *x, const float *parts, int n_parts,
                                                  long long part_stride, const __nv_bfloat16 *res_in,
                                                  const __nv_bfloat16 *w, float eps, int hidden,
@@ -50,24 +62,27 @@ __global__ void __launch_bounds__(512) k_rmsnorm(const __nv_bfloat16 *x, const f
   const int row = blockIdx.x, tid = threadIdx.x;
   const int nvec = hidden >> 3;
   const long long row_off = (long long)row * hidden;
-  const uint4 *rv = res_in ? reinterpret_cast<const uint4 *>(res_in + (long long)row * hidden) : nullptr;
-  uint4 *rov = res_out ? reinterpret_cast<uint4 *>(res_out + (long long)row * hidden) : nullptr;
+  const uint4 *rv = res_in ? reinterpret_cast<const uint4 *>(res_in + row_off) : nullptr;
+  uint4 *rov = res_out ? reinterpret_cast<uint4 *>(res_out + row_off) : nullptr;
   float ss = 0.f;
-  // hidden <= 8 * 512 * 2 : keep up to two vectors per thread in registers
-  Pack8 keep[2];
-  int cnt = 0;
-  for (int v = tid; v < nvec; v += 512) {
-    Pack8 a = load_x8(x, parts, n_parts, part_stride, row_off + v * 8);
-    if (rv) {
-      Pack8 r; r.u = rv[v];
+  // res_in may alias res_out (the decoder layer updates its residual in place): each vector is read before it is
+  // written, by the same thread, and never read again
+  Pack8 keep[kRmsVec];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) a.h[j] = __float2bfloat16_rn(__bfloat162float(a.h[j]) + __bfloat162float(r.h[j]));
+  for (int k = 0; k < kRmsVec; ++k) {
+    const int v = tid + k * 512;
+    if (v < nvec) {
+      Pack8 a = load_x8(x, parts, n_parts, part_stride, row_off + v * 8);
+      if (rv) {
+        Pack8 r; r.u = rv[v];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) a.h[j] = __float2bfloat16_rn(__bfloat162float(a.h[j]) + __bfloat162float(r.h[j]));
+      }
+      if (rov) rov[v] = a.u;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { const float f = __bfloat162float(a.h[j]); ss += f * f; }
+      keep[k] = a;
     }
-    if (rov) rov[v] = a.u;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { const float f = __bfloat162float(a.h[j]); ss += f * f; }
-    if (cnt < 2) keep[cnt] = a;
-    ++cnt;
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(FULL, ss, o);
@@ -78,23 +93,20 @@ __global__ void __launch_bounds__(512) k_rmsnorm(const __nv_bfloat16 *x, const f
   for (int i = 0; i < 16; ++i) tot += red[i];
   const float inv = rsqrtf(tot / (float)hidden + eps);
   const uint4 *wv = reinterpret_cast<const uint4 *>(w);
-  uint4 *yv = reinterpret_cast<uint4 *>(y + (long long)row * hidden);
-  cnt = 0;
-  for (int v = tid; v < nvec; v += 512) {
-    Pack8 a;
-    if (cnt < 2) a = keep[cnt];
-    else {  // (only for hidden > 8192) recompute the residual sum
-      a = load_x8(x, parts, n_parts, part_stride, row_off + v * 8);
-      if (rv) { Pack8 r; r.u = rv[v];
+  uint4 *yv = reinterpret_cast<uint4 *>(y + row_off);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) a.h[j] = __float2bfloat16_rn(__bfloat162float(a.h[j]) + __bfloat162float(r.h[j])); }
+  for (int k = 0; k < kRmsVec; ++k) {
+    const int v = tid + k * 512;
+    if (v < nvec) {
+      Pack8 ww; ww.u = wv[v];
+      Pack8 o;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float xh = __bfloat162float(keep[k].h[j]) * inv;
+        o.h[j] = __float2bfloat16_rn(__bfloat162float(ww.h[j]) * (kRoundTwice ? bf(xh) : xh));
+      }
+      yv[v] = o.u;
     }
-    ++cnt;
-    Pack8 ww; ww.u = wv[v];
-    Pack8 o;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) o.h[j] = __float2bfloat16_rn(__bfloat162float(ww.h[j]) * (__bfloat162float(a.h[j]) * inv));
-    yv[v] = o.u;
   }
 }
 
@@ -329,27 +341,35 @@ __global__ void __launch_bounds__(256) k_bloom_gelu(const __nv_bfloat16 *in, lon
 using namespace pia;
 using namespace pia::fused;
 
-extern "C" int pia_rmsnorm(const void *d_x, const void *d_residual_in, const void *d_weight, float eps, int rows,
-                           int hidden, void *d_residual_out, void *d_y, void *stream) {
-  PIA_REQUIRE(d_x && d_weight && d_y && rows > 0 && hidden > 0 && hidden % 8 == 0, "bad rmsnorm arguments");
-  PIA_CUDA_CHECK(launch_kernel(k_rmsnorm, dim3(rows), dim3(512), 0, (cudaStream_t)stream, (const __nv_bfloat16 *)d_x,
-                              (const float *)nullptr, 0, 0ll, (const __nv_bfloat16 *)d_residual_in,
+static int rmsnorm(const void *d_x, const float *d_parts, int n_parts, long long part_stride, const void *d_residual_in,
+                   const void *d_weight, float eps, int rounding, int rows, int hidden, void *d_residual_out, void *d_y,
+                   void *stream) {
+  PIA_REQUIRE(d_weight && d_y && rows > 0 && hidden > 0 && hidden % 8 == 0 && hidden <= kRmsMaxHidden,
+              "bad rmsnorm arguments: hidden must be a positive multiple of 8, at most 16384");
+  PIA_REQUIRE(rounding == PIA_RMSNORM_ROUND_ONCE || rounding == PIA_RMSNORM_ROUND_TWICE,
+              "bad rmsnorm rounding: PIA_RMSNORM_ROUND_ONCE or PIA_RMSNORM_ROUND_TWICE");
+  auto kern = rounding == PIA_RMSNORM_ROUND_TWICE ? k_rmsnorm<true> : k_rmsnorm<false>;
+  PIA_CUDA_CHECK(launch_kernel(kern, dim3(rows), dim3(512), 0, (cudaStream_t)stream, (const __nv_bfloat16 *)d_x,
+                              d_parts, n_parts, part_stride, (const __nv_bfloat16 *)d_residual_in,
                               (const __nv_bfloat16 *)d_weight, eps, hidden, (__nv_bfloat16 *)d_residual_out,
                               (__nv_bfloat16 *)d_y));
   count_launch();
   return PIA_OK;
 }
 
+extern "C" int pia_rmsnorm(const void *d_x, const void *d_residual_in, const void *d_weight, float eps, int rounding,
+                           int rows, int hidden, void *d_residual_out, void *d_y, void *stream) {
+  PIA_REQUIRE(d_x, "bad rmsnorm arguments");
+  return rmsnorm(d_x, nullptr, 0, 0ll, d_residual_in, d_weight, eps, rounding, rows, hidden, d_residual_out, d_y,
+                 stream);
+}
+
 extern "C" int pia_rmsnorm_partials(const float *d_x_parts, int n_parts, int64_t part_stride, const void *d_residual_in,
-                                    const void *d_weight, float eps, int rows, int hidden, void *d_residual_out,
-                                    void *d_y, void *stream) {
-  PIA_REQUIRE(d_x_parts && n_parts >= 1 && d_weight && d_y && rows > 0 && hidden > 0 && hidden % 8 == 0, "bad rmsnorm arguments");
-  PIA_CUDA_CHECK(launch_kernel(k_rmsnorm, dim3(rows), dim3(512), 0, (cudaStream_t)stream,
-                              (const __nv_bfloat16 *)nullptr, d_x_parts, n_parts, (long long)part_stride,
-                              (const __nv_bfloat16 *)d_residual_in, (const __nv_bfloat16 *)d_weight, eps, hidden,
-                              (__nv_bfloat16 *)d_residual_out, (__nv_bfloat16 *)d_y));
-  count_launch();
-  return PIA_OK;
+                                    const void *d_weight, float eps, int rounding, int rows, int hidden,
+                                    void *d_residual_out, void *d_y, void *stream) {
+  PIA_REQUIRE(d_x_parts && n_parts >= 1, "bad rmsnorm arguments");
+  return rmsnorm(nullptr, d_x_parts, n_parts, (long long)part_stride, d_residual_in, d_weight, eps, rounding, rows,
+                 hidden, d_residual_out, d_y, stream);
 }
 
 template <int kLayout>

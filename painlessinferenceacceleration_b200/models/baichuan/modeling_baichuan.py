@@ -67,6 +67,8 @@ class BaichuanBase(LlamaForCausalLM):
     alibi = False       # Baichuan-13B, Baichuan2-13B: ALiBi instead of RoPE
     norm_head = False   # Baichuan2: L2-normalised lm_head rows
     rope_fp32 = False   # Baichuan2-7B: fp32 cos / sin tables and arithmetic
+    # every member's RMSNorm casts x_hat to bf16, then multiplies by the weight (baichuan_7b/modeling_baichuan.py:84-91)
+    rmsnorm_rounding = ops.ROUND_TWICE
 
     def __init__(self, config, device=None, dtype=torch.bfloat16):
         hd = config.hidden_size // config.num_attention_heads

@@ -17,6 +17,7 @@ import json
 import os
 import types
 
+from ...common import ops
 from ..glm4.modeling_glm4 import GlmForCausalLM
 
 _LAYER = 'transformer.encoder.layers.'
@@ -71,6 +72,9 @@ class ChatGLMForConditionalGeneration(GlmForCausalLM):
     """THUDM-format ChatGLM2/3 checkpoints on the GLM decoder.  Built from a GlmConfig (use from_pretrained(path) for a
     checkpoint directory, or chatglm_config(dict) for a config.json already read); module tree and parameter names
     are transformers' GlmForCausalLM's."""
+    # THUDM's RMSNorm rounds once, (weight * hidden_states).to(input_dtype) (chatglm/modeling_chatglm.py:187,
+    # chatglm3/modeling_chatglm.py:196), unlike transformers' GlmRMSNorm that GlmForCausalLM follows
+    rmsnorm_rounding = ops.ROUND_ONCE
 
     @staticmethod
     def chatglm_config(cfg):

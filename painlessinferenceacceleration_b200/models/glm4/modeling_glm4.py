@@ -19,6 +19,7 @@ any group.  Only the default RoPE type is supported."""
 import torch
 from torch import nn
 
+from ...common import ops
 from ..llama.modeling_llama import Fp8Linear, Fp8Rows, LlamaDecoderLayer, LlamaForCausalLM, LlamaModel, LlamaRMSNorm
 
 
@@ -58,6 +59,7 @@ class GlmForCausalLM(LlamaForCausalLM):
     model_cls = GlmModel
     model_type = 'glm'
     rotary_interleaved = True
+    rmsnorm_rounding = ops.ROUND_TWICE   # transformers' GlmRMSNorm / Glm4RMSNorm: weight * hidden_states.to(input_dtype)
 
     _fp8_params = ('self_attn.q_proj.weight', 'self_attn.k_proj.weight', 'self_attn.v_proj.weight',
                    'self_attn.o_proj.weight', 'mlp.gate_up_proj.weight', 'mlp.down_proj.weight')

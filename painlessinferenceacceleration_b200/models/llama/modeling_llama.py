@@ -144,6 +144,9 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
     model_cls = LlamaModel
     rotary_interleaved = False   # GLM: RoPE on the first geometry()['rotary_dim'] dims of a head, in (2i, 2i+1) pairs
     sandwich_norms = False       # GLM-4-0414: RMSNorm of each sublayer's output before its residual add
+    # where RMSNorm rounds the normalised value: once, bf16(w * x_hat) (llama/modeling_llama.py:90), or twice,
+    # bf16(w * bf16(x_hat)) (the families whose norm casts x_hat to bf16 before the weight multiply; DESIGN.md)
+    rmsnorm_rounding = ops.ROUND_ONCE
 
     def __init__(self, config, device=None, dtype=torch.bfloat16):
         super().__init__(config)
@@ -646,17 +649,19 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         alibi = getattr(rt, 'alibi_slopes', None)   # ALiBi models (Baichuan-13B): the slopes on the device
         x, parts, resid_in = b.h, None, None  # norm(x | parts, resid_in) -> (resid = x + resid_in, y = norm(resid))
 
+        rnd = self.rmsnorm_rounding
+
         def norm(w):
             if parts is not None:
-                ops.rmsnorm_partials(parts, resid_in, w, eps, b.resid, b.y)
+                ops.rmsnorm_partials(parts, resid_in, w, eps, b.resid, b.y, rounding=rnd)
             else:
-                ops.rmsnorm(x, resid_in, w, eps, b.resid, b.y)
+                ops.rmsnorm(x, resid_in, w, eps, b.resid, b.y, rounding=rnd)
 
         def post_norm(w):   # a sublayer output normalised alone (no residual), into b.post_norm
             if parts is not None:
-                ops.rmsnorm_partials(parts, None, w, eps, None, b.post_norm)
+                ops.rmsnorm_partials(parts, None, w, eps, None, b.post_norm, rounding=rnd)
             else:
-                ops.rmsnorm(x, None, w, eps, None, b.post_norm)
+                ops.rmsnorm(x, None, w, eps, None, b.post_norm, rounding=rnd)
             return b.post_norm, None
 
         for li, layer in enumerate(self.model.layers):

@@ -5,6 +5,7 @@ attention kernel packs two query heads of one KV head into each UMMA M=128 tile 
 the reference's lookahead branch - the sliding window is ignored (:979-982 vs :1016-1022)."""
 import warnings
 
+from ...common import ops
 from ..llama.modeling_llama import LlamaForCausalLM
 
 
@@ -20,6 +21,8 @@ def warn_sliding_window(config, max_pos):
 
 
 class MistralForCausalLM(LlamaForCausalLM):
+    rmsnorm_rounding = ops.ROUND_TWICE   # weight * hidden_states.to(input_dtype) (mistral/modeling_mistral.py:90)
+
     def rope_tables(self, max_pos):
         warn_sliding_window(self.config, max_pos)
         return super().rope_tables(max_pos)

@@ -51,6 +51,7 @@ class MixtralModel(LlamaModel):
 
 class MixtralForCausalLM(LlamaForCausalLM):
     model_cls = MixtralModel
+    rmsnorm_rounding = ops.ROUND_TWICE   # weight * hidden_states.to(input_dtype) (mixtral/modeling_mixtral.py:165)
 
     def _fuse_mlp(self, layer):
         pass  # experts are stored fused ([E, 2I, H]) already

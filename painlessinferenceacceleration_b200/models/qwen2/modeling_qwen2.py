@@ -8,6 +8,7 @@ QKV projection stays on cuBLAS (PIA_GEMM_SET=qkv is refused).  Query heads per K
 the tree attention kernel packs them two per tile all the same, the last tile of each KV head holding one.
 As on the reference's lookahead branch, the sliding window is ignored (:997-1000 builds the mask without one; the
 window mask exists only on the non-lookahead branch, :1036-1043)."""
+from ...common import ops
 from ..llama.modeling_llama import LlamaDecoderLayer, LlamaForCausalLM, LlamaModel
 from ..mistral.modeling_mistral import warn_sliding_window
 
@@ -22,6 +23,7 @@ class Qwen2Model(LlamaModel):
 
 class Qwen2ForCausalLM(LlamaForCausalLM):
     model_cls = Qwen2Model
+    rmsnorm_rounding = ops.ROUND_TWICE   # weight * hidden_states.to(input_dtype) (qwen2/modeling_qwen2.py:96)
 
     def rope_tables(self, max_pos):
         # Qwen2 configs carry a `sliding_window` value even when the window is off: only use_sliding_window=True counts

@@ -34,7 +34,8 @@ def test_ctypes_table_matches_header():
     from painlessinferenceacceleration_b200 import _lib
     assert sorted(_lib.SYMBOLS) == _declared()
     L = _lib.load()
-    assert L.pia_abi_version() == 2  # v2: request slots (pia_slots_t), device-resident max_length / idx
+    assert L.pia_abi_version() == 3  # v3: pia_rmsnorm / pia_rmsnorm_partials take the rounding of x_hat
+    # (v2: request slots (pia_slots_t), device-resident max_length / idx)
     assert L.pia_launch_count() == 0
     assert L.pia_last_error() is not None
 

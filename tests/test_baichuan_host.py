@@ -148,4 +148,4 @@ def test_new_symbols_in_header_and_ctypes_table():
         assert name in _lib.SYMBOLS
     assert len(_lib.SYMBOLS['pia_tree_attn_alibi_fwd'][1]) == 9
     assert _lib.SYMBOLS['pia_rope_f32_kv_append'][1] == _lib.SYMBOLS['pia_rope_kv_append'][1]
-    assert '#define PIA_ABI_VERSION 2' in hdr
+    assert '#define PIA_ABI_VERSION 3' in hdr

@@ -179,5 +179,5 @@ def test_new_symbols_in_header_and_ctypes_table():
         assert name in _lib.SYMBOLS
     assert len(_lib.SYMBOLS['pia_layernorm'][1]) == 10
     assert len(_lib.SYMBOLS['pia_bloom_gelu'][1]) == 4
-    assert '#define PIA_ABI_VERSION 2' in hdr
+    assert '#define PIA_ABI_VERSION 3' in hdr
     assert 'bloom/modeling_bloom.py:194-203' in hdr

@@ -1,6 +1,7 @@
 # -*- coding: utf-8 -*-
 """Numerics of the verify-forward kernels against plain PyTorch fp32 restatements of the reference ops
-(models/llama/modeling_llama.py:76-90, 156-169, 185-186, 243-308; pretrained_model.py:764-892, 894-907)."""
+(models/llama/modeling_llama.py:156-169, 185-186, 243-308; pretrained_model.py:764-892, 894-907).  RMSNorm, SiLU*up
+and the embedding gather are tested in depth in tests/test_gpu_norm_power.py."""
 
 import numpy as np
 import pytest
@@ -81,26 +82,6 @@ def test_tree_attention(Hq, Hkv, P, n, pad):
         attn_ref.assert_close(got, ref, f'layer {layer} max abs err {err}')
 
 
-def test_rmsnorm_residual():
-    from painlessinferenceacceleration_b200.common import ops
-    torch.manual_seed(0)
-    for hidden in (256, 4096):
-        x = torch.randn((64, hidden), device=DEV).to(torch.bfloat16)
-        r = torch.randn((64, hidden), device=DEV).to(torch.bfloat16)
-        w = (1 + 0.1 * torch.randn((hidden,), device=DEV)).to(torch.bfloat16)
-        y = torch.empty_like(x)
-        ro = torch.empty_like(x)
-        ops.rmsnorm(x, r, w, 1e-6, ro, y)
-        s = (x.float() + r.float()).to(torch.bfloat16)
-        var = s.float().pow(2).mean(-1, keepdim=True)
-        ref = (w.float() * (s.float() * torch.rsqrt(var + 1e-6))).to(torch.bfloat16)  # modeling_llama.py:85-90
-        assert torch.equal(ro, s)
-        assert torch.allclose(y.float(), ref.float(), atol=1e-2, rtol=1e-2)
-        assert (y != ref).float().mean().item() < 0.01  # only last-bit rounding differences
-        ops.rmsnorm(x, None, w, 1e-6, ro, y)
-        assert torch.equal(ro, x)
-
-
 def test_rope_kv_append_and_silu():
     from painlessinferenceacceleration_b200.common import ops
     torch.manual_seed(1)
@@ -143,12 +124,13 @@ def test_rope_kv_append_and_silu():
     ref2 = (qk * c2) + (rot(qk) * s2)
     assert torch.equal(qo2[:n], ref2[:, :Hq])
     assert torch.equal(kc2[:, 3:3 + n].transpose(0, 1), ref2[:, Hq:])
+    # SiLU(gate) * up equals eager bf16 torch bit for bit (every gate value and the width tails:
+    # tests/test_gpu_norm_power.py)
     gu = torch.randn((64, 2 * 1024), device=DEV).to(torch.bfloat16)
     out = torch.empty((64, 1024), dtype=torch.bfloat16, device=DEV)
     ops.silu_mul(gu, out)
     ref = torch.nn.functional.silu(gu[:, :1024]) * gu[:, 1024:]
-    assert torch.allclose(out.float(), ref.float(), atol=1e-2, rtol=1e-2)
-    assert (out != ref).float().mean().item() < 0.01
+    assert torch.equal(out, ref)
 
 
 def _host_accept(ids, parent, row_tok):
@@ -565,24 +547,6 @@ def test_gemm_weight_streaming(N, K, split):
         torch.cuda.synchronize()
         gemm_ref.assert_close(out[:5], ref[:5], mass[:5], K, 1, '5 rows')
         assert float(out[5:].float().min()) == 7.0
-
-
-def test_rmsnorm_partials_matches_bf16_input():
-    from painlessinferenceacceleration_b200.common import ops
-    torch.manual_seed(3)
-    hidden = 4096
-    parts = torch.randn((4, 64, hidden), device=DEV)
-    r = torch.randn((64, hidden), device=DEV).to(torch.bfloat16)
-    w = (1 + 0.1 * torch.randn((hidden,), device=DEV)).to(torch.bfloat16)
-    x = parts.sum(0).to(torch.bfloat16)
-    y0, r0 = torch.empty_like(r), torch.empty_like(r)
-    y1, r1 = torch.empty_like(r), torch.empty_like(r)
-    ops.rmsnorm(x, r, w, 1e-6, r0, y0)
-    ops.rmsnorm_partials(parts, r, w, 1e-6, r1, y1)
-    torch.cuda.synchronize()
-    # the slice sum is taken in slice order in fp32, like torch's sum over dim 0 of 4 slices up to association
-    assert (r0 != r1).float().mean().item() < 0.02 and (y0 != y1).float().mean().item() < 0.02
-    assert torch.allclose(y0.float(), y1.float(), atol=2e-2, rtol=2e-2)
 
 
 def test_gemm_fused_silu_epilogue_matches_unfused():
