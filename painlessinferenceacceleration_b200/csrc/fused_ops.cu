@@ -454,6 +454,10 @@ extern "C" int pia_bloom_gelu(const void *d_in, int64_t n, void *d_out, void *st
 // MoE combine (mixtral/modeling_mixtral.py:734-759 restated densely): out[t] = sum over experts e, in expert-index
 // order, of ye[e][t] * w[t][e]; the product and every partial sum are rounded to bf16 like the eager bf16 loop
 // (`final_hidden_states.index_add_`), w = 0 for the experts a token did not select.  grid = rows, thread = 8 columns.
+// An expert whose weight is 0 is skipped, not added as ye * 0: the reference never evaluates an unselected expert for
+// the token, so an inf or NaN in that expert's output must not reach out[t] (inf * 0 = NaN).  For finite outputs the
+// skip changes no bit: the accumulator starts at +0, never becomes -0, and adding +-0 leaves it as it is.  It differs
+// from the reference only for a selected expert whose bf16 weight underflowed to 0 and whose output is not finite.
 __global__ void __launch_bounds__(256) k_moe_combine(const __nv_bfloat16 *ye, const __nv_bfloat16 *w, int n_exp, int rows_cap,
                                                      int hidden, __nv_bfloat16 *out) {
   pdl_launch_dependents();
@@ -465,6 +469,7 @@ __global__ void __launch_bounds__(256) k_moe_combine(const __nv_bfloat16 *ye, co
     for (int j = 0; j < 8; ++j) acc.h[j] = __float2bfloat16_rn(0.f);
     for (int e = 0; e < n_exp; ++e) {
       const float we = __bfloat162float(w[(long long)t * n_exp + e]);
+      if (we == 0.f) continue;
       Pack8 y;
       y.u = *reinterpret_cast<const uint4 *>(ye + ((long long)e * rows_cap + t) * hidden + v * 8);
 #pragma unroll
@@ -477,8 +482,8 @@ __global__ void __launch_bounds__(256) k_moe_combine(const __nv_bfloat16 *ye, co
 
 extern "C" int pia_moe_combine(const void *d_expert_out, const void *d_weights, int n_experts, int rows, int rows_cap,
                                int hidden, void *d_out, void *stream) {
-  PIA_REQUIRE(d_expert_out && d_weights && d_out && n_experts > 0 && rows > 0 && rows <= rows_cap && hidden % 8 == 0,
-              "bad combine arguments");
+  PIA_REQUIRE(d_expert_out && d_weights && d_out && n_experts > 0 && rows > 0 && rows <= rows_cap && hidden > 0 &&
+                  hidden % 8 == 0, "bad combine arguments");
   PIA_CUDA_CHECK(launch_kernel(k_moe_combine, dim3(rows), dim3(256), 0, (cudaStream_t)stream,
                               (const __nv_bfloat16 *)d_expert_out, (const __nv_bfloat16 *)d_weights, n_experts, rows_cap,
                               hidden, (__nv_bfloat16 *)d_out));
@@ -534,8 +539,8 @@ __global__ void __launch_bounds__(256) k_moe_router(const __nv_bfloat16 *y, cons
 
 extern "C" int pia_moe_router(const void *d_y, const void *d_gate_weight, int rows, int hidden, int n_experts, int top_k,
                               void *d_dense_out, void *stream) {
-  PIA_REQUIRE(d_y && d_gate_weight && d_dense_out && rows > 0 && hidden % 8 == 0 && n_experts >= 1 && n_experts <= 64 &&
-                  top_k >= 1 && top_k <= n_experts, "bad router arguments");
+  PIA_REQUIRE(d_y && d_gate_weight && d_dense_out && rows > 0 && hidden > 0 && hidden % 8 == 0 && n_experts >= 1 &&
+                  n_experts <= 64 && top_k >= 1 && top_k <= n_experts, "bad router arguments");
   PIA_CUDA_CHECK(launch_kernel(k_moe_router, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const __nv_bfloat16 *)d_y,
                               (const __nv_bfloat16 *)d_gate_weight, hidden, n_experts, top_k, (__nv_bfloat16 *)d_dense_out));
   count_launch();

@@ -8,7 +8,11 @@ either way (SURVEY.md 8d: >= 90 GB per step); the block therefore evaluates ever
 static-shape GEMMs (CUDA-graph friendly, no host-side routing) and combines with the routing weights, zero for
 unselected experts.  Rounding follows the reference: fp32 softmax -> top-k -> renormalise -> cast to bf16 (:723-727);
 per token the two selected expert outputs are scaled in bf16 and accumulated in expert-index order, exactly what
-`index_add_` into a zero tensor produces (:729-757); adding an unselected expert's 0 is exact."""
+`index_add_` into a zero tensor produces (:729-757).  An expert whose bf16 weight for a token is 0 is skipped for that
+token rather than added as `ye * 0`: the reference never evaluates an unselected expert for the token, so an inf or NaN
+in that expert's output must not turn the sum into NaN.  For finite outputs the skip changes no bit (the sum starts at
++0, never becomes -0, and adding +-0 leaves it unchanged).  It differs from the reference only for a selected expert
+whose weight underflowed to 0 in bf16 and whose output is not finite: the reference's sum is then NaN, ours is not."""
 import torch
 from torch import nn
 
@@ -175,5 +179,6 @@ class MixtralForCausalLM(LlamaForCausalLM):
             gu = torch.mm(y, moe.experts.gate_up_proj[e].t())
             ops.silu_mul(gu, act)
             ye = torch.mm(act, moe.experts.down_proj[e].t())
-            out += ye * dense[:, e:e + 1]                                           # bf16 scale, bf16 accumulate
+            w = dense[:, e:e + 1]                                                   # bf16 scale, bf16 accumulate;
+            out += torch.where(w != 0, ye * w, 0.0)                                 # rows that skip e add +0
         return out, None
