@@ -325,6 +325,14 @@ int pia_rope_interleaved_kv_append(const void *d_qkv, const uint64_t *d_mask, in
 int pia_rope_f32_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
                            int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin, int max_pos,
                            void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq, void *stream);
+/* Qwen (v1): pia_rope_f32_kv_append plus log-n attention scaling of the queries (qwen/modeling_qwen.py:223-227,
+ * :374-380, query * logn_tensor after RoPE).  d_q_scale : [max_pos] bf16, read at the row's tree position pos; every
+ * rotated q element becomes bf16(float(bf16(rot)) * float(d_q_scale[pos])).  K and V are written exactly as
+ * pia_rope_f32_kv_append writes them.  All other arguments as pia_rope_f32_kv_append. */
+int pia_rope_f32_logn_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
+                                int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin,
+                                int max_pos, void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq,
+                                const void *d_q_scale, void *stream);
 /* SiLU(gate) * up (modeling_llama.py:185-186). d_gate_up : [rows, 2*inter] (gate | up) -> d_out [rows, inter] */
 int pia_silu_mul(const void *d_gate_up, int rows, int inter, void *d_out, void *stream);
 /* embedding gather for the draft nodes: d_out[i] = table[d_ids[i]] (rows >= *d_n are zero filled) */

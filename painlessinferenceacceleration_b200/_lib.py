@@ -101,6 +101,8 @@ SYMBOLS = {
                                                  vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp]),
     'pia_rope_f32_kv_append': (C.c_int, [vp, vp, C.c_int, C.POINTER(Slots), C.c_int, C.c_int, C.c_int, vp, vp,
                                          C.c_int, vp, vp, vp, C.c_int, vp]),
+    'pia_rope_f32_logn_kv_append': (C.c_int, [vp, vp, C.c_int, C.POINTER(Slots), C.c_int, C.c_int, C.c_int, vp,
+                                              vp, C.c_int, vp, vp, vp, C.c_int, vp, vp]),
     'pia_silu_mul': (C.c_int, [vp, C.c_int, C.c_int, vp, vp]),
     'pia_embed_gather': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     'pia_layernorm': (C.c_int, [vp, vp, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp]),

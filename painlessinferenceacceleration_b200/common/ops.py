@@ -246,18 +246,27 @@ class Slots(object):
 
 
 def rope_kv_append(qkv, mask, slots, n_q_heads, n_kv_heads, head_dim, cos, sin, q_out, k_layer, v_layer, max_seq,
-                   rotary_dim=None):
+                   rotary_dim=None, q_scale=None):
     """qkv / q_out: >= slots.rows rows; mask: [>= slots.rows, W] int64 ancestor rows; k_layer / v_layer: the layer's
     [n_kv_heads, max_seq, head_dim] planes of slot 0.  rotary_dim=None: Llama RoPE over the whole head (tables
     [max_pos, head_dim/2]); an int: GLM RoPE, interleaved pairs over the first rotary_dim dims (tables
     [max_pos, rotary_dim/2]), the rest passed through (pia_rope_interleaved_kv_append).  float32 tables (Llama layout
-    only): fp32 arithmetic, one bf16 rounding (pia_rope_f32_kv_append, Baichuan2-7B)"""
+    only): fp32 arithmetic, one bf16 rounding (pia_rope_f32_kv_append, Baichuan2-7B).  q_scale: a bf16 [max_pos]
+    table the rotated queries are multiplied by at their positions, in bf16 (Qwen's log-n scaling,
+    pia_rope_f32_logn_kv_append; float32 tables only)"""
     assert qkv.shape[0] >= slots.rows and mask.shape[0] >= slots.rows
     assert cos.dtype == sin.dtype and cos.dtype in (torch.bfloat16, torch.float32)
     L_ = L.load()
     args = (_p(qkv), _p(mask), mask.shape[-1], slots.ref(), n_q_heads, n_kv_heads, head_dim, _p(cos), _p(sin),
             cos.shape[0], _p(q_out), _p(k_layer), _p(v_layer), max_seq)
-    if cos.dtype == torch.float32:
+    if q_scale is not None:
+        if cos.dtype != torch.float32 or rotary_dim is not None:
+            raise ValueError('log-n query scaling exists for the fp32 half-split (Qwen) RoPE only')
+        if q_scale.dtype != torch.bfloat16 or q_scale.dim() != 1 or q_scale.shape[0] < cos.shape[0]:
+            raise ValueError(f'q_scale must be bf16 [>= {cos.shape[0]}] (one entry per table position), got '
+                             f'{q_scale.dtype} {tuple(q_scale.shape)}')
+        L.check(L_.pia_rope_f32_logn_kv_append(*args, _p(q_scale), _s()))
+    elif cos.dtype == torch.float32:
         if rotary_dim is not None:
             raise ValueError('fp32 RoPE tables exist for the half-split (Llama) layout only')
         L.check(L_.pia_rope_f32_kv_append(*args, _s()))

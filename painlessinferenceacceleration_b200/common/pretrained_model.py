@@ -223,6 +223,10 @@ class LookaheadPreTrainedModel(nn.Module):
                 self._gemm_plans(rt)
         return rt
 
+    def _start_request(self, rt, input_len, max_length=None):
+        """per-request model state set when a request's prefill starts (`input_len` tokens, left padding included):
+        nothing by default; Qwen fixes its dynamic-NTK RoPE tables here"""
+
     def quantize_fp8(self):
         """fp8 weight-only mode; the Llama family implements it (GPT-2's linears run through torch)"""
         raise NotImplementedError(f'{type(self).__name__} has no fp8 weight mode')
@@ -406,6 +410,7 @@ class LookaheadPreTrainedModel(nn.Module):
                 nz = torch.nonzero(am.to('cpu') != 0)
                 pad_len = int(nz[0]) if nz.numel() else 0
         rt.set_request(0, pad_len, max_length)
+        self._start_request(rt, prompt_len, max_length)
         # multinomial accept (:787-789, :835-837): softmax of the processed scores, no warpers on this path (:430-441)
         sample = bool(decoding_kwargs.get('do_sample', False))
         if sample:
@@ -714,6 +719,8 @@ class LookaheadPreTrainedModel(nn.Module):
         rt.n.fill_(n)
         rt.prefix_len.fill_(P)
         rt.set_request(0, pad_len, 1 << 30)
+        if P == 0:   # no past: a prefill, the request starts here
+            self._start_request(rt, n)
         self._verify_layers(rt)
         logits = rt.logits[:n].clone()[None]
         return logits, P + n

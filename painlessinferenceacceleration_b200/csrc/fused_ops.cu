@@ -117,14 +117,17 @@ __global__ void __launch_bounds__(512) k_rmsnorm(const __nv_bfloat16 *x, const f
 //                   (2i, 2i+1) with frequency i, bf16 tables [max_pos, rotary_dim/2]; the other dims pass through.
 // ROPE_HALF_F32:    Llama layout with fp32 tables [max_pos, hd/2] and fp32 arithmetic, one bf16 rounding at the end
 //                   (baichuan2_7b/modeling_baichuan.py:148-155: q.float() * cos + rotate_half(q.float()) * sin).
+// kLogn (ROPE_HALF_F32 only): Qwen's log-n attention scaling (qwen/modeling_qwen.py:374-380), every rotated q element
+//                   times q_scale[pos] in bf16 arithmetic, bf16(float(bf16(rot)) * float(q_scale[pos])); K / V untouched.
 enum { ROPE_HALF = 0, ROPE_INTERLEAVED = 1, ROPE_HALF_F32 = 2 };
-template <int kLayout>
+template <int kLayout, bool kLogn = false>
 __global__ void __launch_bounds__(256) k_rope_kv_append(const __nv_bfloat16 *qkv, const unsigned long long *mask,
                                                         int mask_words, pia_slots_t sl,
                                                         int hq, int hkv, int hd, const void *cos_t,
                                                         const void *sin_t, int max_pos, __nv_bfloat16 *q_out,
                                                         __nv_bfloat16 *kc, __nv_bfloat16 *vc, int max_seq,
-                                                        int rotary_dim) {
+                                                        int rotary_dim, const __nv_bfloat16 *q_scale) {
+  static_assert(!kLogn || kLayout == ROPE_HALF_F32, "log-n scaling is built on the fp32 layout only");
   pdl_launch_dependents();
   pdl_wait();
   const int i = blockIdx.x;                       // activation row
@@ -183,6 +186,13 @@ __global__ void __launch_bounds__(256) k_rope_kv_append(const __nv_bfloat16 *qkv
           const float x = __bfloat162float(a.h[j]);
           const float r = d0 < half ? -__bfloat162float(b.h[j]) : __bfloat162float(b.h[j]);
           o.h[j] = __float2bfloat16_rn(__fadd_rn(__fmul_rn(x, c[j]), __fmul_rn(r, s[j])));
+        }
+        if constexpr (kLogn) {
+          if (head < hq) {  // query * logn_tensor: a bf16 product of the rounded rotation and the bf16 table entry
+            const float sc = __bfloat162float(q_scale[pos]);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) o.h[j] = __float2bfloat16_rn(__fmul_rn(__bfloat162float(o.h[j]), sc));
+          }
         }
       } else {
         const int dp = d0 < half ? d0 + half : d0 - half;
@@ -372,20 +382,22 @@ extern "C" int pia_rmsnorm_partials(const float *d_x_parts, int n_parts, int64_t
                  hidden, d_residual_out, d_y, stream);
 }
 
-template <int kLayout>
+template <int kLayout, bool kLogn = false>
 static int rope_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
                           int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin, int max_pos,
                           void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq, int rotary_dim,
-                          void *stream) {
+                          void *stream, const void *d_q_scale = nullptr) {
   PIA_REQUIRE(d_qkv && d_mask && slots && slots->d_n && slots->d_prefix_len && d_cos && d_sin && d_q_out &&
                   d_k_cache_layer && d_v_cache_layer, "null argument");
   PIA_REQUIRE(slots->batch >= 1 && slots->rows_per_slot >= 1 && slots->kv_slot_stride >= 0, "bad slot table");
   PIA_REQUIRE(head_dim % 16 == 0 && mask_words >= 1 && mask_words <= 2, "bad rope arguments");
-  PIA_CUDA_CHECK(launch_kernel(k_rope_kv_append<kLayout>, dim3(slots->batch * slots->rows_per_slot), dim3(256), 0,
+  PIA_REQUIRE(!kLogn || d_q_scale, "null argument");
+  PIA_CUDA_CHECK(launch_kernel(k_rope_kv_append<kLayout, kLogn>, dim3(slots->batch * slots->rows_per_slot), dim3(256), 0,
                               (cudaStream_t)stream, (const __nv_bfloat16 *)d_qkv, (const unsigned long long *)d_mask,
                               mask_words, *slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin, max_pos,
                               (__nv_bfloat16 *)d_q_out,
-                              (__nv_bfloat16 *)d_k_cache_layer, (__nv_bfloat16 *)d_v_cache_layer, max_seq, rotary_dim));
+                              (__nv_bfloat16 *)d_k_cache_layer, (__nv_bfloat16 *)d_v_cache_layer, max_seq, rotary_dim,
+                              (const __nv_bfloat16 *)d_q_scale));
   count_launch();
   return PIA_OK;
 }
@@ -404,6 +416,16 @@ extern "C" int pia_rope_f32_kv_append(const void *d_qkv, const uint64_t *d_mask,
                                       int max_seq, void *stream) {
   return rope_kv_append<ROPE_HALF_F32>(d_qkv, d_mask, mask_words, slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin,
                                        max_pos, d_q_out, d_k_cache_layer, d_v_cache_layer, max_seq, head_dim, stream);
+}
+
+extern "C" int pia_rope_f32_logn_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words,
+                                           const pia_slots_t *slots, int n_q_heads, int n_kv_heads, int head_dim,
+                                           const void *d_cos, const void *d_sin, int max_pos, void *d_q_out,
+                                           void *d_k_cache_layer, void *d_v_cache_layer, int max_seq,
+                                           const void *d_q_scale, void *stream) {
+  return rope_kv_append<ROPE_HALF_F32, true>(d_qkv, d_mask, mask_words, slots, n_q_heads, n_kv_heads, head_dim, d_cos,
+                                             d_sin, max_pos, d_q_out, d_k_cache_layer, d_v_cache_layer, max_seq,
+                                             head_dim, stream, d_q_scale);
 }
 
 extern "C" int pia_rope_interleaved_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words,

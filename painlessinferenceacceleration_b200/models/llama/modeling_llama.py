@@ -647,6 +647,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             self._check_fused_attn()
         rotary_dim = g['rotary_dim'] if self.rotary_interleaved else None
         alibi = getattr(rt, 'alibi_slopes', None)   # ALiBi models (Baichuan-13B): the slopes on the device
+        logn = getattr(rt, 'logn_scale', None)      # Qwen's log-n query scaling: a bf16 table on the device
         x, parts, resid_in = b.h, None, None  # norm(x | parts, resid_in) -> (resid = x + resid_in, y = norm(resid))
 
         rnd = self.rmsnorm_rounding
@@ -684,7 +685,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             else:            # prefill chunks share one cache: append first, then attend
                 ops.rope_kv_append(b.qkv, b.mask, b.slots, g['n_q_heads'], g['n_kv_heads'], g['head_dim'], rt.rope_cos,
                                    rt.rope_sin, b.q, rt.k_layer(li, b.kv_slot), rt.v_layer(li, b.kv_slot), rt.max_seq,
-                                   rotary_dim=rotary_dim)
+                                   rotary_dim=rotary_dim, q_scale=logn)
                 rt.plan.forward(li, b.q, b.mask, b.slots, b.attn, alibi_slopes=alibi)
             if lp and 'o' in lp:
                 o = lp['o'].run(rows)
