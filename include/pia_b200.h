@@ -262,6 +262,10 @@ int pia_gemm_plan_set_pdl(pia_gemm_plan_t *g, int on);
 /* fused SiLU(gate) * up epilogue (modeling_llama.py:185-186): the weight must be laid out so that every 128-row tile
  * holds 64 gate rows followed by the 64 up rows of the same columns; d_out of pia_gemm_run is then [rows, N/2]. */
 int pia_gemm_plan_set_silu(pia_gemm_plan_t *g, int on);
+/* fp8 plans only: ReLU in the bias epilogue (OPT's fc1, opt/modeling_opt.py:356), y = bf16(max(acc * s[n] + bias[n],
+ * 0)), one rounding, in the split_k == 1 and the cluster split-K epilogue (after the cluster sum and the bias).
+ * PIA_ERR_INVALID on bf16-weight plans, on plans that write fp32 split-K slices and on plans with set_silu. */
+int pia_gemm_plan_set_relu(pia_gemm_plan_t *g, int on);
 /* splits == 1: d_out is bf16 [rows_cap, N]; splits > 1: d_out is fp32 [splits][64][N] partial slices (sum them in
  * slice order, e.g. with pia_rmsnorm_partials).  rows <= 64 rows are written. */
 int pia_gemm_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream);
@@ -333,11 +337,27 @@ int pia_rope_f32_logn_kv_append(const void *d_qkv, const uint64_t *d_mask, int m
                                 int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin,
                                 int max_pos, void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq,
                                 const void *d_q_scale, void *stream);
+/* OPT (opt/modeling_opt.py:175-181): the KV append without rotation, with the query pre-scaled.  d_qkv : [batch *
+ * rows_per_slot, (Hq + 2*Hkv) * src_head_dim] bf16 (the biased projection output at the checkpoint's head width); q
+ * is written as bf16(float(q) * q_mul) (HF's `q_proj(h) * self.scaling`, the scalar as fp32) to d_q_out [rows, Hq,
+ * head_dim], K and V unchanged to cache rows P_s + i as pia_rope_kv_append; columns [src_head_dim, head_dim) of q / K
+ * / V are written as zeros (heads zero-padded to the attention kernel's width).  No tables are read.  src_head_dim a
+ * positive multiple of 8, at most head_dim, else PIA_ERR_INVALID. */
+int pia_kv_append_qscale(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
+                         int n_q_heads, int n_kv_heads, int src_head_dim, int head_dim, float q_mul, void *d_q_out,
+                         void *d_k_cache_layer, void *d_v_cache_layer, int max_seq, void *stream);
 /* SiLU(gate) * up (modeling_llama.py:185-186). d_gate_up : [rows, 2*inter] (gate | up) -> d_out [rows, inter] */
 int pia_silu_mul(const void *d_gate_up, int rows, int inter, void *d_out, void *stream);
 /* embedding gather for the draft nodes: d_out[i] = table[d_ids[i]] (rows >= *d_n are zero filled) */
 int pia_embed_gather(const void *d_table, const int32_t *d_ids, const int32_t *d_n, int rows, int hidden, void *d_out,
                      void *stream);
+/* learned absolute positions at tree positions (OPT, opt/modeling_opt.py:109-121, :663): d_out[i] = bf16(a[i] +
+ * d_pos_table[offset + pos_i]), pos_i the tree position of pia_rope_kv_append clamped to [0, max_pos); a[i] =
+ * d_tok_table[d_ids[i]], or d_out[i] itself when d_tok_table is NULL (OPT-350m adds positions after project_in).
+ * d_pos_table : [offset + max_pos, hidden] bf16.  Rows past their slot's n are zero filled.  hidden % 8 == 0. */
+int pia_learned_pos_embed(const void *d_tok_table, const int32_t *d_ids, const void *d_pos_table, int offset,
+                          int max_pos, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots, int hidden,
+                          void *d_out, void *stream);
 /* LayerNorm with weight and bias (BLOOM: bloom/modeling_bloom.py input_layernorm / post_attention_layernorm :346-349,
  * word_embeddings_layernorm :422, ln_f :428).  If d_residual_in != NULL: x <- bf16(x + residual_in) first (dropout_add,
  * :504 / :539); x is written to d_residual_out when that is not NULL.  Then y = bf16((x - mean) * rsqrt(var + eps) * w + b)

@@ -94,6 +94,7 @@ SYMBOLS = {
     'pia_gemm_plan_splits': (C.c_int, [vp]),
     'pia_gemm_plan_set_pdl': (C.c_int, [vp, C.c_int]),
     'pia_gemm_plan_set_silu': (C.c_int, [vp, C.c_int]),
+    'pia_gemm_plan_set_relu': (C.c_int, [vp, C.c_int]),
     'pia_gemm_run': (C.c_int, [vp, C.c_int, vp, vp]),
     'pia_rope_kv_append': (C.c_int, [vp, vp, C.c_int, C.POINTER(Slots), C.c_int, C.c_int, C.c_int, vp, vp,
                                      C.c_int, vp, vp, vp, C.c_int, vp]),
@@ -105,6 +106,10 @@ SYMBOLS = {
                                               vp, C.c_int, vp, vp, vp, C.c_int, vp, vp]),
     'pia_silu_mul': (C.c_int, [vp, C.c_int, C.c_int, vp, vp]),
     'pia_embed_gather': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),
+    'pia_kv_append_qscale': (C.c_int, [vp, vp, C.c_int, C.POINTER(Slots), C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_float, vp, vp, vp, C.c_int, vp]),
+    'pia_learned_pos_embed': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, C.c_int, C.POINTER(Slots), C.c_int, vp,
+                                        vp]),
     'pia_layernorm': (C.c_int, [vp, vp, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp]),
     'pia_bloom_gelu': (C.c_int, [vp, C.c_int64, vp, vp]),
     'pia_moe_combine': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),

@@ -207,6 +207,11 @@ class Gemm(object):
         L.check(self.lib.pia_gemm_plan_set_silu(self.h, int(on)))
         return self
 
+    def set_relu(self, on=True):
+        """fp8 plans with bf16 outputs: ReLU after the bias, before the one bf16 rounding (pia_gemm_plan_set_relu)"""
+        L.check(self.lib.pia_gemm_plan_set_relu(self.h, int(on)))
+        return self
+
     def run(self, rows=64, out=None):
         o = out if out is not None else self.out
         L.check(self.lib.pia_gemm_run(self.h, rows, _p(o), _s()))
@@ -274,6 +279,31 @@ def rope_kv_append(qkv, mask, slots, n_q_heads, n_kv_heads, head_dim, cos, sin, 
         L.check(L_.pia_rope_kv_append(*args, _s()))
     else:
         L.check(L_.pia_rope_interleaved_kv_append(*args, int(rotary_dim), _s()))
+
+
+def kv_append(qkv, mask, slots, n_q_heads, n_kv_heads, src_head_dim, head_dim, q_mul, q_out, k_layer, v_layer,
+              max_seq):
+    """the KV append without rotation (OPT, pia_kv_append_qscale): qkv [>= slots.rows, (Hq + 2 Hkv) * src_head_dim];
+    q_out [rows, Hq, head_dim] gets bf16(q * q_mul), K / V go to the cache rows unchanged; columns [src_head_dim,
+    head_dim) of q / K / V are written as zeros"""
+    assert qkv.shape[0] >= slots.rows and mask.shape[0] >= slots.rows
+    assert qkv.shape[-1] == (n_q_heads + 2 * n_kv_heads) * src_head_dim and qkv.is_contiguous()
+    L.check(L.load().pia_kv_append_qscale(_p(qkv), _p(mask), mask.shape[-1], slots.ref(), n_q_heads, n_kv_heads,
+                                          int(src_head_dim), int(head_dim), float(q_mul), _p(q_out), _p(k_layer),
+                                          _p(v_layer), max_seq, _s()))
+
+
+def learned_pos_embed(tok_table, ids, pos_table, offset, mask, slots, out):
+    """out[i] = bf16(a[i] + pos_table[offset + pos_i]) at the rows' tree positions, pos_i clamped to
+    [0, pos_table.shape[0] - offset); a[i] = tok_table[ids[i]], or out[i] itself when tok_table is None
+    (pia_learned_pos_embed).  Rows past their slot's n are zeroed."""
+    hidden = out.shape[-1]
+    assert pos_table.shape[-1] == hidden and pos_table.shape[0] > offset and out.shape[0] >= slots.rows
+    assert tok_table is None or (tok_table.shape[-1] == hidden and ids.shape[0] >= slots.rows)
+    assert mask.shape[0] >= slots.rows
+    L.check(L.load().pia_learned_pos_embed(_p(tok_table), _p(ids) if tok_table is not None else None, _p(pos_table),
+                                           int(offset), pos_table.shape[0] - int(offset), _p(mask), mask.shape[-1],
+                                           slots.ref(), hidden, _p(out), _s()))
 
 
 def _alibi_slopes_f64(n):

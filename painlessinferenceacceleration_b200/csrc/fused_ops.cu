@@ -4,9 +4,11 @@
 //   k_rope_kv_append    :156-169 apply_rotary_pos_emb at the tree positions of :587, and the KV-cache append
 //                       that replaces the reference's per-step torch.cat (:265-268); a second instance rotates in
 //                       the GLM layout (chatglm/modeling_chatglm.py:156-169, positions :815), a third one in fp32
-//                       with fp32 tables (baichuan2_7b/modeling_baichuan.py:148-155)
+//                       with fp32 tables (baichuan2_7b/modeling_baichuan.py:148-155), a fourth one without rotation
+//                       and with OPT's pre-scaled query (opt/modeling_opt.py:175)
 //   k_silu_mul          :185-186
 //   k_embed_gather      :582
+//   k_learned_pos_embed opt/modeling_opt.py:109-121, :663 learned positions at tree positions
 //   k_layernorm         bloom/modeling_bloom.py LayerNorm with weight and bias (+ the residual add, dropout_add)
 //   k_bloom_gelu        bloom/modeling_bloom.py:194-203 bloom_gelu_forward
 // Rounding points follow the reference's bf16 eager arithmetic (each torch op rounds to bf16) so that
@@ -119,14 +121,32 @@ __global__ void __launch_bounds__(512) k_rmsnorm(const __nv_bfloat16 *x, const f
 //                   (baichuan2_7b/modeling_baichuan.py:148-155: q.float() * cos + rotate_half(q.float()) * sin).
 // kLogn (ROPE_HALF_F32 only): Qwen's log-n attention scaling (qwen/modeling_qwen.py:374-380), every rotated q element
 //                   times q_scale[pos] in bf16 arithmetic, bf16(float(bf16(rot)) * float(q_scale[pos])); K / V untouched.
-enum { ROPE_HALF = 0, ROPE_INTERLEAVED = 1, ROPE_HALF_F32 = 2 };
+// ROPE_NONE:        no rotation and no tables (OPT, opt/modeling_opt.py:175): q is written as bf16(float(q) * q_mul),
+//                   one rounding of the bf16 projection output, K / V are appended unchanged.  The source rows hold
+//                   heads of hd_src <= hd elements ([rows, (hq + 2 hkv) * hd_src]); q / K / V are written hd wide, the
+//                   columns [hd_src, hd) zero.
+enum { ROPE_HALF = 0, ROPE_INTERLEAVED = 1, ROPE_HALF_F32 = 2, ROPE_NONE = 3 };
+
+// the tree position of activation row i: rowsum(attention_mask) - 1 (modeling_llama.py:587), i.e. the visible prefix
+// keys [pad_len, P) of its slot + its visible draft keys - 1, clamped to [0, max_pos)
+__device__ __forceinline__ int tree_pos(const unsigned long long *mask, int mask_words, int i, int P, int pad_len,
+                                        int max_pos) {
+  int depth = -1;
+  for (int w = 0; w < mask_words; ++w) depth += __popcll(mask[(long long)i * mask_words + w]);
+  int pos = (P > pad_len ? P - pad_len : 0) + depth;
+  if (pos < 0) pos = 0;
+  if (pos >= max_pos) pos = max_pos - 1;
+  return pos;
+}
+
 template <int kLayout, bool kLogn = false>
 __global__ void __launch_bounds__(256) k_rope_kv_append(const __nv_bfloat16 *qkv, const unsigned long long *mask,
                                                         int mask_words, pia_slots_t sl,
                                                         int hq, int hkv, int hd, const void *cos_t,
                                                         const void *sin_t, int max_pos, __nv_bfloat16 *q_out,
                                                         __nv_bfloat16 *kc, __nv_bfloat16 *vc, int max_seq,
-                                                        int rotary_dim, const __nv_bfloat16 *q_scale) {
+                                                        int rotary_dim, const __nv_bfloat16 *q_scale, int hd_src,
+                                                        float q_mul) {
   static_assert(!kLogn || kLayout == ROPE_HALF_F32, "log-n scaling is built on the fp32 layout only");
   pdl_launch_dependents();
   pdl_wait();
@@ -137,12 +157,26 @@ __global__ void __launch_bounds__(256) k_rope_kv_append(const __nv_bfloat16 *qkv
   if (node >= n) return;
   kc += (long long)slot * sl.kv_slot_stride;
   vc += (long long)slot * sl.kv_slot_stride;
-  int depth = -1;
-  for (int w = 0; w < mask_words; ++w) depth += __popcll(mask[(long long)i * mask_words + w]);
-  // rowsum(attention_mask) - 1 (modeling_llama.py:587): visible prefix keys [pad_len, P) + visible draft keys - 1
-  int pos = (P > pad_len ? P - pad_len : 0) + depth;
-  if (pos < 0) pos = 0;
-  if (pos >= max_pos) pos = max_pos - 1;
+  if constexpr (kLayout == ROPE_NONE) {
+    const int cpr = hd >> 3, cache_row = P + node;
+    const __nv_bfloat16 *src = qkv + (long long)i * (hq + 2 * hkv) * hd_src;
+    for (int c = threadIdx.x; c < (hq + 2 * hkv) * cpr; c += blockDim.x) {
+      const int head = c / cpr, d0 = (c % cpr) * 8;
+      Pack8 a;
+      a.u = d0 < hd_src ? *reinterpret_cast<const uint4 *>(src + head * hd_src + d0) : make_uint4(0, 0, 0, 0);
+      if (head < hq) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) a.h[j] = __float2bfloat16_rn(__fmul_rn(__bfloat162float(a.h[j]), q_mul));
+        *reinterpret_cast<uint4 *>(q_out + ((long long)i * hq + head) * hd + d0) = a.u;
+      } else if (head < hq + hkv) {
+        *reinterpret_cast<uint4 *>(kc + ((long long)(head - hq) * max_seq + cache_row) * hd + d0) = a.u;
+      } else {
+        *reinterpret_cast<uint4 *>(vc + ((long long)(head - hq - hkv) * max_seq + cache_row) * hd + d0) = a.u;
+      }
+    }
+    return;
+  }
+  const int pos = tree_pos(mask, mask_words, i, P, pad_len, max_pos);
   const int half = hd >> 1, cpr = hd >> 3;  // 16-byte chunks per head row
   const int row_elems = (hq + 2 * hkv) * hd;
   const __nv_bfloat16 *src = qkv + (long long)i * row_elems;
@@ -245,6 +279,35 @@ __global__ void __launch_bounds__(256) k_embed_gather(const __nv_bfloat16 *table
   if (row >= n) { for (int v = threadIdx.x; v < nvec; v += 256) dst[v] = make_uint4(0, 0, 0, 0); return; }
   const uint4 *src = reinterpret_cast<const uint4 *>(table + (long long)ids[row] * hidden);
   for (int v = threadIdx.x; v < nvec; v += 256) dst[v] = src[v];
+}
+
+// learned absolute positions at tree positions (OPT, opt/modeling_opt.py:109-121 and :663): out[i] = bf16(a[i] +
+// pos_table[offset + pos(i)]), one rounding of the bf16 + bf16 sum as eager `inputs_embeds + pos_embeds`; pos(i) is
+// k_rope_kv_append's tree position, clamped to [0, max_pos).  a[i] = tok[ids[i]], or out[i] itself when tok is null
+// (the row already holds project_in's output).  grid = slot rows; rows past their slot's n are zero, as in
+// k_embed_gather.
+__global__ void __launch_bounds__(256) k_learned_pos_embed(const __nv_bfloat16 *tok, const int *ids,
+                                                           const __nv_bfloat16 *pos_table, int offset, int max_pos,
+                                                           const unsigned long long *mask, int mask_words,
+                                                           pia_slots_t sl, int hidden, __nv_bfloat16 *out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = blockIdx.x;
+  const int slot = i / sl.rows_per_slot, node = i % sl.rows_per_slot;
+  const int nvec = hidden >> 3;
+  uint4 *dst = reinterpret_cast<uint4 *>(out + (long long)i * hidden);
+  if (node >= sl.d_n[slot]) { for (int v = threadIdx.x; v < nvec; v += 256) dst[v] = make_uint4(0, 0, 0, 0); return; }
+  const int pos = tree_pos(mask, mask_words, i, sl.d_prefix_len[slot], sl.d_pad_len ? sl.d_pad_len[slot] : 0, max_pos);
+  const uint4 *src = tok ? reinterpret_cast<const uint4 *>(tok + (long long)ids[i] * hidden) : dst;
+  const uint4 *pe = reinterpret_cast<const uint4 *>(pos_table + (long long)(offset + pos) * hidden);
+  for (int v = threadIdx.x; v < nvec; v += 256) {
+    Pack8 a, p;
+    a.u = src[v];
+    p.u = pe[v];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a.h[j] = __float2bfloat16_rn(__bfloat162float(a.h[j]) + __bfloat162float(p.h[j]));
+    dst[v] = a.u;
+  }
 }
 
 // LayerNorm with weight and bias (bloom/modeling_bloom.py:346-349, :422, :428) over one row per CTA, preceded by the
@@ -386,18 +449,45 @@ template <int kLayout, bool kLogn = false>
 static int rope_kv_append(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
                           int n_q_heads, int n_kv_heads, int head_dim, const void *d_cos, const void *d_sin, int max_pos,
                           void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq, int rotary_dim,
-                          void *stream, const void *d_q_scale = nullptr) {
-  PIA_REQUIRE(d_qkv && d_mask && slots && slots->d_n && slots->d_prefix_len && d_cos && d_sin && d_q_out &&
-                  d_k_cache_layer && d_v_cache_layer, "null argument");
+                          void *stream, const void *d_q_scale = nullptr, int hd_src = 0, float q_mul = 1.f) {
+  PIA_REQUIRE(d_qkv && d_mask && slots && slots->d_n && slots->d_prefix_len && d_q_out && d_k_cache_layer &&
+                  d_v_cache_layer && (kLayout == ROPE_NONE || (d_cos && d_sin)), "null argument");
   PIA_REQUIRE(slots->batch >= 1 && slots->rows_per_slot >= 1 && slots->kv_slot_stride >= 0, "bad slot table");
   PIA_REQUIRE(head_dim % 16 == 0 && mask_words >= 1 && mask_words <= 2, "bad rope arguments");
   PIA_REQUIRE(!kLogn || d_q_scale, "null argument");
+  PIA_REQUIRE(kLayout != ROPE_NONE || (hd_src >= 8 && hd_src % 8 == 0 && hd_src <= head_dim),
+              "bad source head width: a positive multiple of 8, at most head_dim");
   PIA_CUDA_CHECK(launch_kernel(k_rope_kv_append<kLayout, kLogn>, dim3(slots->batch * slots->rows_per_slot), dim3(256), 0,
                               (cudaStream_t)stream, (const __nv_bfloat16 *)d_qkv, (const unsigned long long *)d_mask,
                               mask_words, *slots, n_q_heads, n_kv_heads, head_dim, d_cos, d_sin, max_pos,
                               (__nv_bfloat16 *)d_q_out,
                               (__nv_bfloat16 *)d_k_cache_layer, (__nv_bfloat16 *)d_v_cache_layer, max_seq, rotary_dim,
-                              (const __nv_bfloat16 *)d_q_scale));
+                              (const __nv_bfloat16 *)d_q_scale, hd_src, q_mul));
+  count_launch();
+  return PIA_OK;
+}
+
+extern "C" int pia_kv_append_qscale(const void *d_qkv, const uint64_t *d_mask, int mask_words, const pia_slots_t *slots,
+                                    int n_q_heads, int n_kv_heads, int src_head_dim, int head_dim, float q_mul,
+                                    void *d_q_out, void *d_k_cache_layer, void *d_v_cache_layer, int max_seq,
+                                    void *stream) {
+  return rope_kv_append<ROPE_NONE>(d_qkv, d_mask, mask_words, slots, n_q_heads, n_kv_heads, head_dim, nullptr, nullptr,
+                                   1, d_q_out, d_k_cache_layer, d_v_cache_layer, max_seq, head_dim, stream, nullptr,
+                                   src_head_dim, q_mul);
+}
+
+extern "C" int pia_learned_pos_embed(const void *d_tok_table, const int32_t *d_ids, const void *d_pos_table,
+                                     int offset, int max_pos, const uint64_t *d_mask, int mask_words,
+                                     const pia_slots_t *slots, int hidden, void *d_out, void *stream) {
+  PIA_REQUIRE(d_pos_table && d_mask && slots && slots->d_n && slots->d_prefix_len && d_out &&
+                  (d_ids || !d_tok_table), "null argument");
+  PIA_REQUIRE(slots->batch >= 1 && slots->rows_per_slot >= 1, "bad slot table");
+  PIA_REQUIRE(hidden > 0 && hidden % 8 == 0 && offset >= 0 && max_pos >= 1 && mask_words >= 1 && mask_words <= 2,
+              "bad position embedding arguments: hidden a positive multiple of 8, offset >= 0, max_pos >= 1");
+  PIA_CUDA_CHECK(launch_kernel(k_learned_pos_embed, dim3(slots->batch * slots->rows_per_slot), dim3(256), 0,
+                              (cudaStream_t)stream, (const __nv_bfloat16 *)d_tok_table, (const int *)d_ids,
+                              (const __nv_bfloat16 *)d_pos_table, offset, max_pos, (const unsigned long long *)d_mask,
+                              mask_words, *slots, hidden, (__nv_bfloat16 *)d_out));
   count_launch();
   return PIA_OK;
 }

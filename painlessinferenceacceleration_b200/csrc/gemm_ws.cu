@@ -518,11 +518,16 @@ struct F8Params {
   long long out_group_stride;  // elements between the groups' [x_rows, N] outputs
   long long slice_stride;      // fp32 split-K slices: elements between two splits' [x_rows, N] slices
   int cluster, silu, no_pdl;
+  int relu;                    // 1: y = max(acc * s[n] + bias[n], 0) before the bf16 rounding (bf16 outputs only)
   const float *scale;          // [groups * N], one per stored weight row
   const float *bias;           // [N] or null (split_k == 1 or cluster splits only)
   __nv_bfloat16 *out_bf16;
   float *out_f32;
 };
+
+// the bf16 epilogue's activation: OPT's fc1 ReLU (opt/modeling_opt.py:356) on the biased fp32 value, so that the one
+// bf16 rounding of relu(x) equals relu of the rounded x (bf16 rounding is monotone and keeps 0)
+__device__ __forceinline__ float f8_act(float v, int relu) { return relu ? fmaxf(v, 0.f) : v; }
 
 // NSTAGE = 3: ~106 KB of shared memory, two CTAs per SM; NSTAGE = 6: ~202 KB, one CTA per SM (grids that do not
 // fill the SMs twice) - 96 KB of weight bytes in flight per SM either way
@@ -672,10 +677,10 @@ k_gemm_fp8(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CU
           a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
         }
         const int tt = 4 * tq;
-        if (tt < rows) ob[(long long)tt * p.N + n_out] = __float2bfloat16_rn(a.x + bs);
-        if (tt + 1 < rows) ob[(long long)(tt + 1) * p.N + n_out] = __float2bfloat16_rn(a.y + bs);
-        if (tt + 2 < rows) ob[(long long)(tt + 2) * p.N + n_out] = __float2bfloat16_rn(a.z + bs);
-        if (tt + 3 < rows) ob[(long long)(tt + 3) * p.N + n_out] = __float2bfloat16_rn(a.w + bs);
+        if (tt < rows) ob[(long long)tt * p.N + n_out] = __float2bfloat16_rn(f8_act(a.x + bs, p.relu));
+        if (tt + 1 < rows) ob[(long long)(tt + 1) * p.N + n_out] = __float2bfloat16_rn(f8_act(a.y + bs, p.relu));
+        if (tt + 2 < rows) ob[(long long)(tt + 2) * p.N + n_out] = __float2bfloat16_rn(f8_act(a.z + bs, p.relu));
+        if (tt + 3 < rows) ob[(long long)(tt + 3) * p.N + n_out] = __float2bfloat16_rn(f8_act(a.w + bs, p.relu));
       }
     }
   } else if (p.silu) {
@@ -710,7 +715,7 @@ k_gemm_fp8(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CU
     __nv_bfloat16 *ob = p.out_bf16 + grp * p.out_group_stride + (long long)t0 * p.N;
 #pragma unroll
     for (int t = 0; t < TOK; ++t)
-      if (t < rows) ob[(long long)t * p.N + n] = __float2bfloat16_rn(v[t] + bs);
+      if (t < rows) ob[(long long)t * p.N + n] = __float2bfloat16_rn(f8_act(v[t] + bs, p.relu));
   } else {
     float *o = p.out_f32 + split * p.slice_stride + (long long)t0 * p.N;
 #pragma unroll
@@ -883,11 +888,21 @@ extern "C" int pia_gemm_plan_set_silu(pia_gemm_plan_t *g, int on) {
   if (g && g->fp8) {
     PIA_REQUIRE(g->f.n_split == 1 && !g->f.bias && g->groups == 1,
                 "the SiLU*up epilogue needs split_k == 1, no bias and one group");
+    PIA_REQUIRE(!on || !g->f.relu, "a plan has one epilogue activation: ReLU is already set");
     g->f.silu = on ? 1 : 0;
     return PIA_OK;
   }
   PIA_REQUIRE(g && g->p.n_split == 1 && !g->stream_k && g->p.N % BMW == 0, "the SiLU*up epilogue needs split_k == 1 and N %% 128 == 0");
   g->p.silu = on ? 1 : 0;
+  return PIA_OK;
+}
+extern "C" int pia_gemm_plan_set_relu(pia_gemm_plan_t *g, int on) {
+  PIA_REQUIRE(g && g->fp8, "the ReLU epilogue exists on fp8 plans only");
+  if (on) {
+    PIA_REQUIRE(g->f.n_split == 1 || g->f.cluster, "the ReLU epilogue needs bf16 outputs: split_k == 1 or a cluster split");
+    PIA_REQUIRE(!g->f.silu, "a plan has one epilogue activation: SiLU*up is already set");
+  }
+  g->f.relu = on ? 1 : 0;
   return PIA_OK;
 }
 
@@ -962,7 +977,7 @@ static int f8_plan_create(const void *d_w, const void *d_scale, const void *d_bi
   f.x_group_chunks = groups > 1 ? n_chunks : 0;
   f.out_group_stride = (long long)x_rows * N;
   f.slice_stride = (long long)x_rows * N;
-  f.cluster = 0; f.silu = 0; f.no_pdl = 0;
+  f.cluster = 0; f.silu = 0; f.no_pdl = 0; f.relu = 0;
   f.scale = (const float *)d_scale; f.bias = (const float *)d_bias;
   f.out_bf16 = nullptr; f.out_f32 = nullptr;
   if (want_cluster && f.n_split != want_cluster) { delete g; set_error("K = %d is too short for %d cluster splits", K, want_cluster); return PIA_ERR_INVALID; }
