@@ -283,6 +283,17 @@ int pia_gemm_plan_create_fp8(const void *d_w, const void *d_scale, const void *d
  * d_scale [groups * N]; out[g] ([x_rows, N] bf16, consecutive) = X[:, g*K : (g+1)*K] @ W[g]^T. */
 int pia_gemm_plan_create_grouped_fp8(const void *d_w, const void *d_scale, int groups, int N, int K, const void *d_x,
                                      int x_rows, pia_gemm_plan_t **out);
+/* 4-bit weight-only variant (GPTQ / compressed-tensors pack-quantized checkpoints of the same projections):
+ *   Y[t, n] = sum_k X[t, k] W[n, k] (+ bias[n]),  W[n, k] = bf16(dtype_s(s[g, n] * (u[n, k] - z[g, n]))),  g = k / group,
+ * fp32 accumulate, one bf16 rounding of Y; u the unsigned 4-bit code, z its zero point (0..16), s the group scale in
+ * the checkpoint's dtype (scale_dtype 0: bf16, 1: fp16, which is rounded to fp16 first, then to bf16).  d_codes holds u
+ * tiled as [N/128][ceil(K/256)] contiguous blocks of 128 rows x 128 bytes, nibbles permuted inside every 16-byte group
+ * (ops.tile_weight_w4); d_scale [K/group, N] 16-bit, d_zero [K/group, N] uint8.  N % 128 == 0, K % 128 == 0, group a
+ * multiple of 128 dividing K.  d_bias, split_k, rows and the fp32 slices as for pia_gemm_plan_create_fp8; set_silu /
+ * set_pdl / splits apply, set_relu does not. */
+int pia_gemm_plan_create_w4(const void *d_codes, const void *d_scale, const void *d_zero, int scale_dtype,
+                            const void *d_bias, int N, int K, int group_size, const void *d_x, int x_rows, int split_k,
+                            pia_gemm_plan_t **out);
 
 /* ============================================================================================
  * Fused elementwise pieces of the verify forward (all bf16 I/O, fp32 math)

@@ -118,6 +118,101 @@ def untile_weight_fp8(t):
     return b.permute(0, 1, 3, 2, 4, 5).reshape(*lead, nt * 128, kt * 128).contiguous().view(torch.float8_e4m3fn)
 
 
+# position p (a nibble, low half of its byte first) of every 16-byte group of a tiled int4 weight holds k =
+# _W4_KPERM[p] of the group's 32: word c (bytes 4c..4c+3) is thread c's, its nibble j holds k 2c + (0, 8, 16, 24)[j % 4]
+# + j // 4, so that word >> 8t and word >> (8t + 4), masked with 0x000F000F, are the k pairs of the thread's a0 and a2
+# fragment registers of the group's k-step t
+_W4_KPERM = tuple(2 * c + (0, 8, 16, 24)[j % 4] + j // 4 for c in range(4) for j in range(8))
+W4_SCALE_DTYPES = (torch.bfloat16, torch.float16)
+
+
+def dequantize_w4(u, s, z, group_size):
+    """the weight the int4 GEMM multiplies with, W[n, k] = bf16(dtype_s(s[n, g] * (u[n, k] - z[n, g]))), g = k // group:
+    u uint8 [N, K] codes 0..15, s [N, G] bf16 or fp16, z uint8 [N, G] zero points (the unpackers' form).  u - z is exact
+    in the scale's dtype, the product is rounded once to it (as compressed-tensors' dequantisation does), then to bf16."""
+    N, K = u.shape
+    rep = lambda t: t.repeat_interleave(group_size, dim=1)[:, :K]
+    return ((u.to(s.dtype) - rep(z).to(s.dtype)) * rep(s)).to(torch.bfloat16)
+
+
+def tile_weight_w4(u):
+    """int4 codes uint8 [N, K] (values 0..15) -> uint8 [N/128, ceil(K/256), 128, 128] contiguous (the int4 GEMM's HBM
+    layout): one 16 KB block per (128-row tile, 256-wide k chunk), two codes per byte, nibbles permuted inside every
+    16-byte group by _W4_KPERM; a K that is an odd multiple of 128 is padded with zero codes the kernel never reads"""
+    N, K = u.shape
+    if N % 128 or K % 128:
+        raise ValueError(f'the int4 GEMM needs both weight dimensions to be multiples of 128, got [{N}, {K}]')
+    if K % 256:
+        u = torch.cat([u, u.new_zeros((N, 128))], dim=1)
+    kc = u.shape[1] // 256
+    b = u.reshape(N // 128, 128, kc, 8, 32).index_select(4, torch.tensor(_W4_KPERM, device=u.device))
+    b = (b[..., 0::2] | (b[..., 1::2] << 4)).to(torch.uint8)
+    return b.permute(0, 2, 1, 3, 4).reshape(N // 128, kc, 128, 128).contiguous()
+
+
+def untile_weight_w4(t, K):
+    """inverse of tile_weight_w4: uint8 [N/128, ceil(K/256), 128, 128] -> codes uint8 [N, K]"""
+    nt, kc = t.shape[:2]
+    inv = torch.empty(32, dtype=torch.long)
+    inv[torch.tensor(_W4_KPERM)] = torch.arange(32)
+    b = t.reshape(nt, kc, 128, 8, 16)
+    nib = torch.stack([b & 15, b >> 4], dim=-1).reshape(nt, kc, 128, 8, 32).index_select(4, inv.to(t.device))
+    return nib.permute(0, 2, 1, 3, 4).reshape(nt * 128, kc * 256)[:, :K].contiguous()
+
+
+def _unpack_nibbles(packed, dim):
+    """int32 tensor with 8 nibbles per element (nibble i at bits 4i) -> uint8 codes, the 8 nibbles of an element
+    consecutive along `dim` (0 or 1)"""
+    p = packed.to(torch.int32)
+    nib = torch.stack([(p >> (4 * i)) & 15 for i in range(8)], dim=dim + 1)   # [..., 8] next to the packed dim
+    shape = list(p.shape)
+    shape[dim] *= 8
+    return nib.reshape(shape).to(torch.uint8)
+
+
+def unpack_compressed_tensors_w4(weight_packed, weight_scale, weight_shape=None, weight_zero_point=None):
+    """compressed-tensors `pack-quantized` (num_bits 4): weight_packed int32 [N, K/8] (nibble i of column j is k = 8j + i,
+    stored as the signed code + 8), weight_scale [N, G] (G = 1: channel-wise), weight_zero_point None (symmetric: z = 8)
+    or int32 [ceil(N/8), G] packed along N, stored zp + 8 (an int8 [N, G] tensor of signed zero points is taken too).
+    Returns the internal form (u uint8 [N, K], s [N, G] in the scale's dtype, z uint8 [N, G], group size)."""
+    N = weight_packed.shape[0]
+    K = int(weight_shape[1]) if weight_shape is not None else weight_packed.shape[1] * 8
+    u = _unpack_nibbles(weight_packed, 1)[:, :K].contiguous()
+    s = weight_scale
+    if s.dim() == 1:
+        s = s[:, None]
+    if s.dtype not in W4_SCALE_DTYPES:
+        raise ValueError(f'weight_scale dtype {s.dtype}: the int4 GEMM takes bf16 or fp16 scales')
+    G = s.shape[1]
+    if s.shape[0] != N or K % G:
+        raise ValueError(f'weight_scale {tuple(s.shape)} does not fit a [{N}, {K}] weight')
+    if weight_zero_point is None:
+        z = torch.full((N, G), 8, dtype=torch.uint8, device=u.device)
+    elif weight_zero_point.dtype == torch.int32:
+        z = _unpack_nibbles(weight_zero_point, 0)[:N].contiguous()
+    else:
+        z = (weight_zero_point.to(torch.int16) + 8).to(torch.uint8).reshape(N, G)
+    return u, s.contiguous(), z, K // G
+
+
+def unpack_gptq_w4(qweight, qzeros, scales, g_idx=None):
+    """GPTQ 4-bit, checkpoint_format v1: qweight int32 [K/8, N] packed along K (nibble i of row j is k = 8j + i),
+    qzeros int32 [G, N/8] packed along N, stored z - 1, scales [G, N], g_idx [K] (must be k // group: no act-order).
+    Returns the internal form (u uint8 [N, K], s [N, G], z uint8 [N, G], group size)."""
+    u = _unpack_nibbles(qweight, 0).t().contiguous()
+    N, K = u.shape
+    G = scales.shape[0]
+    if scales.shape[1] != N or K % G:
+        raise ValueError(f'scales {tuple(scales.shape)} do not fit a [{N}, {K}] weight')
+    if scales.dtype not in W4_SCALE_DTYPES:
+        raise ValueError(f'scales dtype {scales.dtype}: the int4 GEMM takes bf16 or fp16 scales')
+    gs = K // G
+    if g_idx is not None and not torch.equal(g_idx.to(torch.long).cpu(), torch.arange(K) // gs):
+        raise ValueError('g_idx is not k // group_size (act-order / desc_act GPTQ): not supported')
+    z = ((_unpack_nibbles(qzeros, 1)[:, :N].to(torch.int16) + 1)).to(torch.uint8).t().contiguous()
+    return u, scales.t().contiguous(), z, gs
+
+
 class Gemm(object):
     """pia_gemm_plan_t: Y = X @ W^T for one (weight, activation buffer) pair; `out` is bf16 [rows, N] when the plan
     has one K split, else fp32 [splits, 64, N]"""
@@ -173,6 +268,36 @@ class Gemm(object):
                                                       split_k, C.byref(self.h)))
         self.splits = self.lib.pia_gemm_plan_splits(self.h)
         self.N, self.weight, self._keep = N, qweight, (qweight, scale, bias, x)
+        if out is not None:
+            self.out = out
+        elif self.splits == 1:
+            self.out = torch.empty((x.shape[0], N), dtype=torch.bfloat16, device=x.device)
+        else:
+            self.out = torch.empty((self.splits, x.shape[0], N), dtype=torch.float32, device=x.device)
+        return self
+
+    @classmethod
+    def w4(cls, codes, scale_t, zero_t, group_size, x, bias=None, split_k=1, out=None):
+        """int4 weight plan (pia_gemm_plan_create_w4): codes = tile_weight_w4(u) of an [N, K] weight, scale_t [K/group, N]
+        bf16 or fp16 and zero_t uint8 [K/group, N] (the unpackers' s and z transposed, same row order), bias fp32 [N] or
+        None; runs 1..x.shape[0] rows; out as for fp8()"""
+        G, N = scale_t.shape
+        K = G * group_size
+        assert codes.dtype == torch.uint8 and codes.is_contiguous() and codes.dim() == 4
+        assert tuple(codes.shape) == (N // 128, -(-K // 256), 128, 128)
+        assert scale_t.dtype in W4_SCALE_DTYPES and scale_t.is_contiguous()
+        assert zero_t.dtype == torch.uint8 and tuple(zero_t.shape) == (G, N) and zero_t.is_contiguous()
+        assert x.shape[1] == K and x.is_contiguous()
+        assert bias is None or (bias.dtype == torch.float32 and bias.numel() == N and bias.is_contiguous())
+        self = cls.__new__(cls)
+        self.lib = L.load()
+        self.h = L.vp()
+        with torch.cuda.device(codes.device):
+            L.check(self.lib.pia_gemm_plan_create_w4(_p(codes), _p(scale_t), _p(zero_t),
+                                                     int(scale_t.dtype == torch.float16), _p(bias), N, K,
+                                                     int(group_size), _p(x), x.shape[0], split_k, C.byref(self.h)))
+        self.splits = self.lib.pia_gemm_plan_splits(self.h)
+        self.N, self.weight, self._keep = N, codes, (codes, scale_t, zero_t, bias, x)
         if out is not None:
             self.out = out
         elif self.splits == 1:

@@ -724,6 +724,286 @@ k_gemm_fp8(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CU
   }
 }
 
+// ------------------------------------------------------------------------------------------------ int4 weights
+// W4A16 with group-wise scales and zero points (GPTQ / compressed-tensors pack-quantized checkpoints): the weight is
+//   W[n, k] = bf16(dtype_s(s[g, n] * (u[n, k] - z[g, n]))),  g = k / group,
+// u the unsigned 4-bit code, z its zero point (0..16), s the group's scale in the checkpoint's dtype (bf16 or fp16).
+// Same structure as k_gemm_fp8 (swap-AB, two consumer warpgroups x wgmma M = 64 over 128 weight rows, TMA producer warp
+// over an mbarrier ring, HBM-tiled weight, gridDim.z over 64-row token blocks), but a stage covers 256 k: one 16 KB
+// block of 128 rows x 128 bytes of codes (ops.tile_weight_w4, one SWIZZLE_128B row per weight row), the four matching
+// 64-k bf16 X boxes, and the scales and zero points of the stage's two 128-k halves (four bulk copies out of the
+// [G, N] tables: 128 rows x {bf16|fp16} and 128 rows x uint8 per half).  The consumers dequantise their wgmma A fragment
+// in registers: a nibble pair becomes (B + u) as a 16-bit pair (B = 128 in bf16, 1024 in fp16, both with ulp 1), minus
+// (B + z) is exact, times s in the scale's own 16-bit arithmetic is the one rounding to dtype_s; fp16 then goes to bf16
+// (a second rounding, as the checkpoint's dequantisation does).  W is bf16 before the MMA, so the epilogue has no scale:
+// k_gemm_fp8's with the multiply removed (bias in fp32, SiLU*up, cluster split-K, fp32 slices).
+constexpr int W4_BK = 256;                                 // k per stage: 128 bytes of packed codes per weight row
+constexpr int W4_W_BYTES = BMW * W4_BK / 2;                // 16 KB
+constexpr int W4_X_OFF = W4_W_BYTES;                       // four 64-k bf16 X boxes, 1024-byte aligned
+constexpr int W4_META_OFF = W4_X_OFF + 4 * X_BYTES;        // scales [2 halves][128] 16-bit, zeros [2 halves][128] u8
+constexpr int W4_STAGE_BYTES = W4_META_OFF + 1024;         // 49 KB: the 768 meta bytes padded to keep stages aligned
+constexpr int w4_smem_total(int nstage) { return nstage * W4_STAGE_BYTES + 256 + XCH_BYTES + 1024; }
+static_assert(ACC_OFF + BMW * ACC_LD * 4 <= 2 * W4_STAGE_BYTES, "accumulator staging must fit in the pipeline stages");
+
+struct W4Params {
+  int N, K, n_chunks, chunks_per_split, n_split, rows, ntb;  // n_chunks: ceil(K / 256); ntb: 64-row token blocks
+  int tiles, group;            // N / 128, k per scale group (a multiple of 128)
+  long long slice_stride;      // fp32 split-K slices: elements between two splits' [x_rows, N] slices
+  int cluster, silu, no_pdl;
+  const void *scale;           // [K / group, N] bf16 or fp16
+  const uint8_t *zero;         // [K / group, N] zero points 0..16
+  const float *bias;           // [N] or null
+  __nv_bfloat16 *out_bf16;
+  float *out_f32;
+};
+
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+// the nibbles at bits [0, 4) and [16, 20) of w -> a bf16x2 fragment register (low half = lower k).  zo = (B + z) in
+// both halves, sc = s in both halves, in the scale's format.
+template <bool F16>
+__device__ __forceinline__ uint32_t w4_deq(uint32_t w, uint32_t zo, uint32_t sc) {
+  uint32_t x = (w & 0x000F000Fu) | (F16 ? 0x64006400u : 0x43004300u), d;
+  if (F16) {
+    asm("{\n\t.reg .b32 t;\n\tsub.rn.f16x2 t, %1, %2;\n\tmul.rn.f16x2 %0, t, %3;\n\t}" : "=r"(d) : "r"(x), "r"(zo), "r"(sc));
+    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&d));
+    const __nv_bfloat162 b = __floats2bfloat162_rn(f.x, f.y);
+    return *reinterpret_cast<const uint32_t *>(&b);
+  }
+  asm("{\n\t.reg .b32 t;\n\tsub.rn.bf16x2 t, %1, %2;\n\tmul.rn.bf16x2 %0, t, %3;\n\t}" : "=r"(d) : "r"(x), "r"(zo), "r"(sc));
+  return d;
+}
+
+// NSTAGE = 2: ~107 KB of shared memory, two CTAs per SM; NSTAGE = 4: ~205 KB, one CTA per SM (grids that do not fill
+// the SMs twice) - 64 KB of code bytes (128 K weights) in flight per SM either way
+template <int NSTAGE, bool F16>
+__global__ void __launch_bounds__(NTHREADS, NSTAGE <= 2 ? 2 : 1)
+k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, W4Params p) {
+  constexpr int SMEM_BAR = NSTAGE * W4_STAGE_BYTES;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t bar_full = base + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE;
+  const int tile = p.cluster ? blockIdx.y : blockIdx.x, split = p.cluster ? blockIdx.x : blockIdx.y;
+  const int n0 = tile * BMW;
+  const int t0 = blockIdx.z * TOK;  // first token row of this CTA
+  const int rows = p.rows - t0 < TOK ? p.rows - t0 : TOK;
+  const int c0 = split * p.chunks_per_split;
+  int c1 = c0 + p.chunks_per_split;
+  if (c1 > p.n_chunks) c1 = p.n_chunks;
+  const int nch = c1 - c0;
+  const int khalves = p.K / 128;    // a last chunk may hold one 128-k half only (K % 256 == 128)
+
+  if (tid == 0) {
+    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncwarp();
+  if (!p.no_pdl) pdl_launch_dependents();
+  __syncthreads();
+
+  if (warp == PRODUCER_WARP) {
+    if (lane == 0) {
+      // codes, scales and zero points are immutable: the first NSTAGE stages stream before griddepcontrol.wait
+      const int wblk = tile * p.n_chunks + c0;
+      constexpr int sb = 2;  // bytes per scale (bf16 or fp16)
+      auto halves = [&](int i) { return 2 * (c0 + i) + 1 < khalves ? 2 : 1; };
+      auto stage_bytes = [&](int i) { return (uint32_t)(W4_W_BYTES + halves(i) * (2 * X_BYTES + BMW * (sb + 1))); };
+      auto load_w = [&](int i, int s) {
+        const uint32_t st = base + s * W4_STAGE_BYTES, bar = bar_full + 8 * s;
+        tma_load_3d(st, &map_w, bar, 0, 0, wblk + i);
+        for (int h = 0; h < halves(i); ++h) {
+          const long long g = (long long)((c0 + i) * W4_BK + h * 128) / p.group;
+          bulk_load(st + W4_META_OFF + h * BMW * sb,
+                    reinterpret_cast<const uint8_t *>(p.scale) + (g * p.N + n0) * sb, BMW * sb, bar);
+          bulk_load(st + W4_META_OFF + 2 * BMW * sb + h * BMW, p.zero + g * p.N + n0, BMW, bar);
+        }
+      };
+      auto load_x = [&](int i, int s) {
+        const uint32_t xd = base + s * W4_STAGE_BYTES + W4_X_OFF;
+        for (int b = 0; b < 2 * halves(i); ++b) tma_load_2d(xd + b * X_BYTES, &map_x, bar_full + 8 * s, ((c0 + i) * 4 + b) * BK, t0);
+      };
+      const int pre = nch < NSTAGE ? nch : NSTAGE;
+      for (int i = 0; i < pre; ++i) {
+        mbar_expect_tx(bar_full + 8 * i, stage_bytes(i));
+        load_w(i, i);
+      }
+      pdl_wait();
+      for (int i = 0; i < pre; ++i) load_x(i, i);
+      for (int i = pre; i < nch; ++i) {
+        const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
+        mbar_wait(bar_empty + 8 * s, ph ^ 1);
+        mbar_expect_tx(bar_full + 8 * s, stage_bytes(i));
+        load_w(i, s);
+        load_x(i, s);
+      }
+    }
+    __syncwarp();
+    if (p.cluster) { cluster_sync_all(); cluster_sync_all(); }
+    return;
+  }
+
+  // ---------------------------------------------------------------- consumers: warpgroup wg owns weight rows [64 wg, +64)
+  pdl_wait();
+  const int wg = warp >> 2;
+  // A fragment of m64k16 as in k_gemm_fp8: a0 = (row r, k 2c..2c+1), a1 = (r + 8, same k), a2 = (r, k + 8),
+  // a3 = (r + 8, k + 8), r = 16 (warp % 4) + lane / 4, c = lane % 4.  Every 16-byte group (32 k) of a tiled row holds one
+  // 32-bit word per c; nibble j of word c is k = 2c + {0, 8, 16, 24}[j % 4] + (j / 4) (ops.tile_weight_w4), so
+  // word >> 8t (t = the k-step inside the group) masked with 0x000F000F is a0's pair, word >> (8t + 4) a2's.  The
+  // 16-byte group j of row r sits at chunk j ^ (r % 8) (SWIZZLE_128B); rows r and r + 8 share that pattern.
+  const int r = wg * 64 + 16 * (warp & 3) + (lane >> 2);
+  const uint32_t roff = (uint32_t)r * 128 + 4 * (lane & 3);
+  const int sw = r & 7;
+  const uint32_t zbase = F16 ? 0x6400u : 0x4300u;
+  float acc[32];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+  for (int i = 0; i < nch; ++i) {
+    const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
+    mbar_wait(bar_full + 8 * s, ph);
+    const uint8_t *ws = sm + s * W4_STAGE_BYTES;
+    const uint16_t *ss = reinterpret_cast<const uint16_t *>(ws + W4_META_OFF);
+    const uint8_t *zz = ws + W4_META_OFF + 4 * BMW;
+    const uint32_t xa = base + s * W4_STAGE_BYTES + W4_X_OFF;
+    const int nh = 2 * (c0 + i) + 1 < khalves ? 2 : 1;
+    for (int h = 0; h < nh; ++h) {
+      uint32_t sc[2], zo[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const uint32_t sv = ss[h * BMW + r + 8 * e], zv = zbase | zz[h * BMW + r + 8 * e];
+        sc[e] = sv | (sv << 16);
+        zo[e] = zv | (zv << 16);
+      }
+      uint32_t a[32];
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const uint32_t off = roff + ((uint32_t)((4 * h + jj) ^ sw) << 4);
+        const uint32_t w0 = *reinterpret_cast<const uint32_t *>(ws + off);
+        const uint32_t w1 = *reinterpret_cast<const uint32_t *>(ws + off + 8 * 128);
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+          a[8 * jj + 4 * t + 0] = w4_deq<F16>(w0 >> (8 * t), zo[0], sc[0]);
+          a[8 * jj + 4 * t + 1] = w4_deq<F16>(w1 >> (8 * t), zo[1], sc[1]);
+          a[8 * jj + 4 * t + 2] = w4_deq<F16>(w0 >> (8 * t + 4), zo[0], sc[0]);
+          a[8 * jj + 4 * t + 3] = w4_deq<F16>(w1 >> (8 * t + 4), zo[1], sc[1]);
+        }
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 8; ++j) wgmma_m64n64k16_ra(acc, a + 4 * j, kmajor_desc(xa + (2 * h + (j >> 2)) * X_BYTES + (j & 3) * 32));
+      wgmma_commit();
+      wgmma_wait_all();
+      fence_acc(acc);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+  }
+  float *accs = reinterpret_cast<float *>(sm + ACC_OFF);
+  asm volatile("bar.sync 2, 256;" ::: "memory");
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int rr = wg * 64 + frag_row(warp, lane, h);
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<float2 *>(accs + rr * ACC_LD + frag_tok(lane, i)) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+  }
+  asm volatile("bar.sync 2, 256;" ::: "memory");
+  if (wg == 1) {
+    if (p.cluster) { cluster_sync_all(); cluster_sync_all(); }
+    return;
+  }
+
+  // epilogue (warps 0-3): thread = one weight row n, its 64 token values
+  const int q = warp;
+  const int n = n0 + q * 32 + lane;
+  float v[64];
+  {
+    const float4 *src = reinterpret_cast<const float4 *>(accs + (q * 32 + lane) * ACC_LD);
+#pragma unroll
+    for (int t = 0; t < 16; ++t) {
+      const float4 a = src[t];
+      v[4 * t] = a.x; v[4 * t + 1] = a.y; v[4 * t + 2] = a.z; v[4 * t + 3] = a.w;
+    }
+  }
+  if (p.cluster) {
+    const int cs = p.cluster, RS = BMW / cs;
+    cluster_sync_all();
+    {
+      const int row = q * 32 + lane;
+      const int owner = row / RS, rl = row % RS;
+      const uint32_t dst = map_to_cta(base + (uint32_t)((split * 16) * RS + rl) * 16, owner);
+#pragma unroll
+      for (int tq = 0; tq < 16; ++tq) st_cluster_f4(dst + (uint32_t)(tq * RS) * 16, v[4 * tq], v[4 * tq + 1], v[4 * tq + 2], v[4 * tq + 3]);
+    }
+    cluster_sync_all();
+    {
+      const int e = warp * 32 + lane;
+      const int rl = e % RS, tg = e / RS;
+      const int qpt = RS / 8;
+      const int n_out = n0 + split * RS + rl;
+      const float4 *buf = reinterpret_cast<const float4 *>(sm);
+      __nv_bfloat16 *ob = p.out_bf16 + (long long)t0 * p.N;
+      for (int tq = tg * qpt; tq < (tg + 1) * qpt; ++tq) {
+        float4 a = buf[(0 * 16 + tq) * RS + rl];
+        for (int src = 1; src < cs; ++src) {
+          const float4 b = buf[(src * 16 + tq) * RS + rl];
+          a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        }
+        if (p.bias) { const float bs = p.bias[n_out]; a.x += bs; a.y += bs; a.z += bs; a.w += bs; }
+        const int tt = 4 * tq;
+        if (tt < rows) ob[(long long)tt * p.N + n_out] = __float2bfloat16_rn(a.x);
+        if (tt + 1 < rows) ob[(long long)(tt + 1) * p.N + n_out] = __float2bfloat16_rn(a.y);
+        if (tt + 2 < rows) ob[(long long)(tt + 2) * p.N + n_out] = __float2bfloat16_rn(a.z);
+        if (tt + 3 < rows) ob[(long long)(tt + 3) * p.N + n_out] = __float2bfloat16_rn(a.w);
+      }
+    }
+  } else if (p.silu) {
+    __nv_bfloat16 *xu = reinterpret_cast<__nv_bfloat16 *>(sm + SMEM_BAR + 256);
+    __nv_bfloat16 *xg = xu + 32 * 64;
+    const int rr = (q & 1) * 32 + lane;
+    if (q >= 2) {
+#pragma unroll
+      for (int t = 0; t < 32; ++t) xu[t * 64 + rr] = __float2bfloat16_rn(v[t]);
+    } else {
+#pragma unroll
+      for (int t = 0; t < 32; ++t) xg[t * 64 + rr] = __float2bfloat16_rn(v[32 + t]);
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    const int col = tile * 64 + rr;
+    const int inter = p.N >> 1;
+    __nv_bfloat16 *ob = p.out_bf16 + (long long)t0 * inter;
+    const int tb = q < 2 ? 0 : 32;
+#pragma unroll
+    for (int t = 0; t < 32; ++t) {
+      if (tb + t < rows) {
+        const float g = q < 2 ? __bfloat162float(__float2bfloat16_rn(v[t])) : __bfloat162float(xg[t * 64 + rr]);
+        const float u = q < 2 ? __bfloat162float(xu[t * 64 + rr]) : __bfloat162float(__float2bfloat16_rn(v[32 + t]));
+        const float sg = __bfloat162float(__float2bfloat16_rn(g / (1.f + expf(-g))));
+        ob[(long long)(tb + t) * inter + col] = __float2bfloat16_rn(sg * u);
+      }
+    }
+  } else if (p.n_split == 1) {
+    // no bias: the accumulator is rounded as it is (k_gemm_ws's epilogue; + 0.f would turn a -0 into +0)
+    if (p.bias) {
+      const float bs = p.bias[n];
+#pragma unroll
+      for (int t = 0; t < TOK; ++t) v[t] += bs;
+    }
+    __nv_bfloat16 *ob = p.out_bf16 + (long long)t0 * p.N;
+#pragma unroll
+    for (int t = 0; t < TOK; ++t)
+      if (t < rows) ob[(long long)t * p.N + n] = __float2bfloat16_rn(v[t]);
+  } else {
+    float *o = p.out_f32 + split * p.slice_stride + (long long)t0 * p.N;
+#pragma unroll
+    for (int t = 0; t < TOK; ++t)
+      if (t < rows) o[(long long)t * p.N + n] = v[t];
+  }
+}
+
 }  // namespace gemm
 }  // namespace pia
 
@@ -741,6 +1021,9 @@ struct pia_gemm_plan {
   // fp8 weight mode (pia_gemm_plan_create_fp8 / _grouped_fp8): k_gemm_fp8 with `f`, up to x_rows rows per run
   int fp8, groups, x_rows;
   F8Params f;
+  // int4 weight mode (pia_gemm_plan_create_w4): k_gemm_w4 with `w`, up to x_rows rows per run
+  int w4, w4_f16;
+  W4Params w;
 };
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -882,6 +1165,7 @@ extern "C" int pia_gemm_plan_set_pdl(pia_gemm_plan_t *g, int on) {
 }
 extern "C" int pia_gemm_plan_splits(const pia_gemm_plan_t *g) {
   if (g && g->fp8) return g->f.cluster ? 1 : g->f.n_split;
+  if (g && g->w4) return g->w.cluster ? 1 : g->w.n_split;
   return g ? (g->p.cluster ? 1 : g->p.n_split) : 0;
 }
 extern "C" int pia_gemm_plan_set_silu(pia_gemm_plan_t *g, int on) {
@@ -890,6 +1174,11 @@ extern "C" int pia_gemm_plan_set_silu(pia_gemm_plan_t *g, int on) {
                 "the SiLU*up epilogue needs split_k == 1, no bias and one group");
     PIA_REQUIRE(!on || !g->f.relu, "a plan has one epilogue activation: ReLU is already set");
     g->f.silu = on ? 1 : 0;
+    return PIA_OK;
+  }
+  if (g && g->w4) {
+    PIA_REQUIRE(g->w.n_split == 1 && !g->w.bias, "the SiLU*up epilogue needs split_k == 1 and no bias");
+    g->w.silu = on ? 1 : 0;
     return PIA_OK;
   }
   PIA_REQUIRE(g && g->p.n_split == 1 && !g->stream_k && g->p.N % BMW == 0, "the SiLU*up epilogue needs split_k == 1 and N %% 128 == 0");
@@ -1010,6 +1299,63 @@ extern "C" int pia_gemm_plan_create_grouped_fp8(const void *d_w, const void *d_s
   return f8_plan_create(d_w, d_scale, nullptr, groups, N, K, d_x, x_rows, 1, out);
 }
 
+// int4 codes, tiled by ops.tile_weight_w4: [N/128][ceil(K/256)] contiguous 16 KB blocks of 128 rows x 128 bytes (256
+// nibbles), one SWIZZLE_128B TMA box each
+static int w4_plan_create(const void *d_codes, const void *d_scale, const void *d_zero, int scale_f16,
+                          const void *d_bias, int N, int K, int group, const void *d_x, int x_rows, int split_k,
+                          pia_gemm_plan_t **out) {
+  PIA_REQUIRE(d_codes && d_scale && d_zero && d_x && out, "null argument");
+  PIA_REQUIRE(N > 0 && N % BMW == 0 && K > 0 && K % 128 == 0, "the int4 GEMM needs N %% %d == 0 and K %% 128 == 0", BMW);
+  PIA_REQUIRE(group > 0 && group % 128 == 0 && K % group == 0, "group size %d: a multiple of 128 that divides K = %d", group, K);
+  PIA_REQUIRE(scale_f16 == 0 || scale_f16 == 1, "scale dtype: 0 = bf16, 1 = fp16");
+  PIA_REQUIRE(x_rows >= TOK, "the activation buffer must hold at least %d rows", TOK);
+  PIA_REQUIRE(((reinterpret_cast<uintptr_t>(d_codes) | reinterpret_cast<uintptr_t>(d_scale) |
+                reinterpret_cast<uintptr_t>(d_zero) | reinterpret_cast<uintptr_t>(d_x)) & 15) == 0,
+              "operands must be 16-byte aligned");
+  const int n_chunks = (K + W4_BK - 1) / W4_BK;
+  const int want_cluster = (split_k == -2 || split_k == -4 || split_k == -8) ? -split_k : 0;
+  PIA_REQUIRE(split_k >= 1 || want_cluster, "int4 plans take split_k >= 1 or a cluster split of 2, 4 or 8 CTAs");
+  if (want_cluster) split_k = want_cluster;
+  if (split_k > n_chunks) split_k = n_chunks;
+  W4Params w;
+  w.N = N; w.K = K; w.n_chunks = n_chunks; w.tiles = N / BMW; w.group = group;
+  w.chunks_per_split = (n_chunks + split_k - 1) / split_k;
+  w.n_split = (n_chunks + w.chunks_per_split - 1) / w.chunks_per_split;
+  w.rows = TOK; w.ntb = 1;
+  w.slice_stride = (long long)x_rows * N;
+  w.cluster = 0; w.silu = 0; w.no_pdl = 0;
+  w.scale = d_scale; w.zero = (const uint8_t *)d_zero; w.bias = (const float *)d_bias;
+  w.out_bf16 = nullptr; w.out_f32 = nullptr;
+  if (want_cluster && w.n_split != want_cluster) { set_error("K = %d is too short for %d cluster splits", K, want_cluster); return PIA_ERR_INVALID; }
+  w.cluster = want_cluster;
+  if (d_bias && w.n_split > 1 && !w.cluster) { set_error("a bias needs split_k == 1 or a cluster split"); return PIA_ERR_INVALID; }
+  pia_gemm_plan *g = new (std::nothrow) pia_gemm_plan();
+  PIA_REQUIRE(g, "out of host memory");
+  g->w = w; g->w4 = 1; g->w4_f16 = scale_f16; g->groups = 1; g->x_rows = x_rows;
+  int rc = encode_tiled_w_fp8(&g->map_w, d_codes, (uint64_t)w.tiles * n_chunks);   // the same 128 x 128-byte boxes
+  if (rc == PIA_OK) rc = encode_2d(&g->map_x, d_x, (uint64_t)K, (uint64_t)x_rows, BK, TOK, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc == PIA_OK) {
+    int n_sm = 132, dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    g->nstage = w.tiles * w.n_split <= n_sm ? 4 : 2;
+    cudaError_t e = cudaFuncSetAttribute(k_gemm_w4<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(2));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(4));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(2));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(4));
+    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); rc = PIA_ERR_CUDA; }
+  }
+  if (rc != PIA_OK) { delete g; return rc; }
+  *out = g;
+  return PIA_OK;
+}
+
+extern "C" int pia_gemm_plan_create_w4(const void *d_codes, const void *d_scale, const void *d_zero, int scale_dtype,
+                                       const void *d_bias, int N, int K, int group_size, const void *d_x, int x_rows,
+                                       int split_k, pia_gemm_plan_t **out) {
+  return w4_plan_create(d_codes, d_scale, d_zero, scale_dtype, d_bias, N, K, group_size, d_x, x_rows, split_k, out);
+}
+
 struct PdlScope { int on; explicit PdlScope(int off) : on(off) { if (on) ++pia::g_pdl_off; } ~PdlScope() { if (on) --pia::g_pdl_off; } };
 
 static int f8_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream) {
@@ -1027,9 +1373,30 @@ static int f8_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream) {
   return PIA_OK;
 }
 
+static int w4_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream) {
+  PIA_REQUIRE(rows >= 1 && rows <= g->x_rows, "rows %d outside [1,%d]", rows, g->x_rows);
+  PdlScope pdl_scope(g->no_pdl);
+  W4Params w = g->w;
+  w.rows = rows; w.ntb = (rows + TOK - 1) / TOK; w.no_pdl = g->no_pdl;
+  if (w.n_split == 1 || w.cluster) w.out_bf16 = (__nv_bfloat16 *)d_out; else w.out_f32 = (float *)d_out;
+  const dim3 grid = w.cluster ? dim3(w.n_split, w.tiles, w.ntb) : dim3(w.tiles, w.n_split, w.ntb);
+  const unsigned cs = w.cluster ? (unsigned)w.cluster : 1u;
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (g->nstage == 4) {
+    if (g->w4_f16) PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_w4<4, true>, grid, dim3(NTHREADS), w4_smem_total(4), st, cs, g->map_w, g->map_x, w));
+    else PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_w4<4, false>, grid, dim3(NTHREADS), w4_smem_total(4), st, cs, g->map_w, g->map_x, w));
+  } else {
+    if (g->w4_f16) PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_w4<2, true>, grid, dim3(NTHREADS), w4_smem_total(2), st, cs, g->map_w, g->map_x, w));
+    else PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_w4<2, false>, grid, dim3(NTHREADS), w4_smem_total(2), st, cs, g->map_w, g->map_x, w));
+  }
+  count_launch();
+  return PIA_OK;
+}
+
 extern "C" int pia_gemm_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream) {
   PIA_REQUIRE(g && d_out, "null argument");
   if (g->fp8) return f8_run(g, rows, d_out, stream);
+  if (g->w4) return w4_run(g, rows, d_out, stream);
   PIA_REQUIRE(rows >= 1 && rows <= TOK, "rows %d outside [1,%d]", rows, TOK);
   PdlScope pdl_scope(g->no_pdl);
   if (g->stream_k) {

@@ -64,6 +64,7 @@ def baichuan_config(cfg):
 class BaichuanBase(LlamaForCausalLM):
     """shared base of the four Baichuan classes; module tree and parameter names are Llama's (the checkpoint's
     W_pack is split into q / k / v on load)"""
+    int4_checkpoints = False   # quantization_config is refused by the config check
     alibi = False       # Baichuan-13B, Baichuan2-13B: ALiBi instead of RoPE
     norm_head = False   # Baichuan2: L2-normalised lm_head rows
     rope_fp32 = False   # Baichuan2-7B: fp32 cos / sin tables and arithmetic

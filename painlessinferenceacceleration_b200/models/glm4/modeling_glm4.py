@@ -57,6 +57,7 @@ class Glm4Model(LlamaModel):
 
 class GlmForCausalLM(LlamaForCausalLM):
     model_cls = GlmModel
+    int4_checkpoints = False   # no int4 weight mode for this family
     model_type = 'glm'
     rotary_interleaved = True
     rmsnorm_rounding = ops.ROUND_TWICE   # transformers' GlmRMSNorm / Glm4RMSNorm: weight * hidden_states.to(input_dtype)

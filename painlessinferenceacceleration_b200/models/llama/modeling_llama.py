@@ -112,6 +112,123 @@ class Fp8Rows(nn.Module):
         return q.float() * s.unsqueeze(-1)
 
 
+class Int4Linear(nn.Module):
+    """4-bit weight of one projection, as a GPTQ / compressed-tensors checkpoint stores it, in the int4 GEMM's layout:
+    `qweight` uint8 (ops.tile_weight_w4 of the codes), `scale` [G, N] in the checkpoint's scale dtype, `zero` uint8
+    [G, N] zero points (G = K / group_size).  `interleaved`: a fused gate/up weight whose rows (with their scales and zero
+    points) are stored in the SiLU*up epilogue's order."""
+
+    def __init__(self, u, s, z, group_size, interleaved=False):
+        super().__init__()
+        self.shape = tuple(u.shape)
+        self.group_size = int(group_size)
+        self.interleaved = interleaved
+        if interleaved:
+            u, s, z = _gate_up_order(u), _gate_up_order(s), _gate_up_order(z)
+        self.qweight = nn.Parameter(ops.tile_weight_w4(u), requires_grad=False)
+        self.scale = nn.Parameter(s.t().contiguous(), requires_grad=False)
+        self.zero = nn.Parameter(z.t().contiguous(), requires_grad=False)
+
+    def codes(self):
+        """(u uint8 [N, K], s [N, G], z uint8 [N, G]) in the checkpoint's row order"""
+        u = ops.untile_weight_w4(self.qweight, self.shape[1])
+        s, z = self.scale.data.t(), self.zero.data.t()
+        if self.interleaved:
+            u, s, z = (_gate_up_order(t, inverse=True) for t in (u, s, z))
+        return u, s.contiguous(), z.contiguous()
+
+    def dequantize(self):
+        """the weight the int4 GEMM multiplies with (ops.dequantize_w4), bf16 [N, K]"""
+        return ops.dequantize_w4(*self.codes(), self.group_size)
+
+    def gemm(self, x, **kw):
+        return ops.Gemm.w4(self.qweight, self.scale, self.zero, self.group_size, x, **kw)
+
+
+class Int4Rows(Fp8Rows):
+    """rows [r0, r1) of a fused Int4Linear under their HF name; `bias` (Qwen2) stays the bf16 parameter it was"""
+
+    def codes(self):
+        u, s, z = self._fused[0].codes()
+        return u[self.r0:self.r1], s[self.r0:self.r1], z[self.r0:self.r1]
+
+    def dequantize(self):
+        return ops.dequantize_w4(*self.codes(), self._fused[0].group_size)
+
+
+def _w4_spec(config):
+    """the int4 layout a checkpoint's quantization_config describes -> dict(format='gptq' | 'compressed-tensors',
+    group_size (None: channel-wise), sym); ValueError naming the field for anything the int4 GEMM does not run"""
+    q = getattr(config, 'quantization_config', None)
+    q = q.to_dict() if hasattr(q, 'to_dict') else dict(q)
+    method = q.get('quant_method')
+    if method == 'gptq':
+        if q.get('bits') != 4:
+            raise ValueError(f'quantization_config.bits={q.get("bits")!r}: only 4-bit GPTQ checkpoints are supported')
+        if q.get('desc_act'):
+            raise ValueError('quantization_config.desc_act=True: act-order GPTQ checkpoints are not supported')
+        if (q.get('checkpoint_format') or 'gptq') != 'gptq':
+            raise ValueError(f'quantization_config.checkpoint_format={q.get("checkpoint_format")!r}: only the v1 '
+                             "'gptq' format (zero points stored minus one) is supported")
+        if q.get('lm_head'):
+            raise ValueError('quantization_config.lm_head=True: a quantised lm_head is not supported')
+        gs, sym = q.get('group_size', 128), q.get('sym', True)
+    elif method == 'compressed-tensors':
+        if q.get('format') != 'pack-quantized':
+            raise ValueError(f'quantization_config.format={q.get("format")!r}: only compressed-tensors '
+                             "'pack-quantized' int4 checkpoints are supported")
+        groups = list((q.get('config_groups') or {}).values())
+        if not groups:
+            raise ValueError('quantization_config.config_groups is empty')
+        w = groups[0].get('weights') or {}
+        for g in groups:
+            if g.get('weights') != w:
+                raise ValueError('quantization_config.config_groups: groups with different weight schemes are not '
+                                 'supported')
+            if g.get('input_activations') is not None:
+                raise ValueError('quantization_config.config_groups.input_activations: only weight-only (W4A16) '
+                                 'checkpoints are supported')
+            if g.get('targets') != ['Linear']:
+                raise ValueError(f'quantization_config.config_groups.targets={g.get("targets")!r}: only Linear targets '
+                                 'are supported')
+        if w.get('num_bits') != 4:
+            raise ValueError(f'quantization_config weights.num_bits={w.get("num_bits")!r}: only 4-bit weights are '
+                             'supported')
+        if w.get('type', 'int') != 'int':
+            raise ValueError(f'quantization_config weights.type={w.get("type")!r}: only int weights are supported')
+        if w.get('actorder') not in (None, False):
+            raise ValueError(f'quantization_config weights.actorder={w.get("actorder")!r}: act-order is not supported')
+        strategy = w.get('strategy')
+        if strategy not in ('group', 'channel'):
+            raise ValueError(f'quantization_config weights.strategy={strategy!r}: only group and channel are supported')
+        if w.get('dynamic'):
+            raise ValueError('quantization_config weights.dynamic=True is not supported')
+        ignore = q.get('ignore') or []
+        if not any(i == 'lm_head' or (i.startswith('re:') and 'lm_head' in i) for i in ignore):
+            raise ValueError(f'quantization_config.ignore={ignore!r} does not hold lm_head: a quantised lm_head is not '
+                             'supported')
+        gs, sym = (w.get('group_size') if strategy == 'group' else -1), w.get('symmetric', True)
+    else:
+        raise ValueError(f'quantization_config.quant_method={method!r}: only gptq and compressed-tensors '
+                         '(pack-quantized) 4-bit checkpoints are supported')
+    if gs in (None, -1):
+        gs = None
+    elif int(gs) <= 0 or int(gs) % 128:
+        raise ValueError(f'quantization_config group_size={gs}: the int4 GEMM takes groups of a multiple of 128 '
+                         'weights (or channel-wise scales)')
+    c = config
+    hd = c.hidden_size // c.num_attention_heads
+    kv = getattr(c, 'num_key_value_heads', None) or c.num_attention_heads
+    for field, v in (('hidden_size', c.hidden_size), ('intermediate_size', c.intermediate_size),
+                     ('num_attention_heads * head_dim', c.num_attention_heads * hd),
+                     ('num_key_value_heads * head_dim', kv * hd)):
+        if v % 128:
+            raise ValueError(f'{field}={v}: int4 weights need every projection dimension divisible by 128')
+        if gs is not None and field in ('hidden_size', 'intermediate_size') and v % int(gs):
+            raise ValueError(f'{field}={v} is not a multiple of quantization_config group_size={gs}')
+    return dict(format=method, group_size=int(gs) if gs is not None else None, sym=bool(sym))
+
+
 class LlamaDecoderLayer(nn.Module):
     qkv_bias = False   # biases on q/k/v (Qwen2); o_proj never has one
 
@@ -147,6 +264,9 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
     # where RMSNorm rounds the normalised value: once, bf16(w * x_hat) (llama/modeling_llama.py:90), or twice,
     # bf16(w * bf16(x_hat)) (the families whose norm casts x_hat to bf16 before the weight multiply; DESIGN.md)
     rmsnorm_rounding = ops.ROUND_ONCE
+    # whether from_pretrained reads GPTQ / compressed-tensors int4 checkpoints (the Llama decoder's projections);
+    # families that refuse or ignore quantization_config set False
+    int4_checkpoints = True
 
     def __init__(self, config, device=None, dtype=torch.bfloat16):
         super().__init__(config)
@@ -157,6 +277,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         self.lm_head = nn.Linear(config.hidden_size, config.vocab_size, bias=False, device=device, dtype=dtype)
         self._fused = False
         self._fp8 = False
+        self._w4 = False
         for p_ in self.parameters():  # inference only: no autograd state on the hot path
             p_.requires_grad_(False)
 
@@ -185,10 +306,17 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
     def from_pretrained(cls, path, torch_dtype=torch.bfloat16, device=None, quantization=None, **kwargs):
         """HF checkpoint directory (config.json + *.safetensors / pytorch_model*.bin) -> model on the GPU.
         quantization='fp8': the decoder projections become fp8 weights as they arrive (see quantize_fp8); the bf16
-        decoder never exists on the GPU."""
+        decoder never exists on the GPU.  A GPTQ or compressed-tensors int4 checkpoint (config.quantization_config) is
+        loaded as it is stored, one layer at a time, onto the int4 GEMM (see _w4_spec for what is accepted)."""
         if quantization not in (None, 'fp8'):
             raise ValueError(f'quantization={quantization!r}: only None and \'fp8\' are supported')
         config = cls._pretrained_config(path)
+        if cls.int4_checkpoints and getattr(config, 'quantization_config', None):
+            spec = _w4_spec(config)
+            if quantization is not None:
+                raise ValueError(f'quantization={quantization!r}: this checkpoint is already quantised '
+                                 f'({spec["format"]} int4); load it with quantization=None')
+            return cls._from_pretrained_w4(path, config, spec, device)
         if quantization == 'fp8':
             return cls._from_pretrained_fp8(path, config, device)
         model = cls(config, device=device, dtype=torch_dtype)
@@ -300,6 +428,157 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         model._fp8 = True
         return model
 
+    # ------------------------------------------------------------------ int4 (GPTQ / compressed-tensors) weights
+    _W4_PARTS = {'compressed-tensors': ('weight_packed', 'weight_scale', 'weight_shape', 'weight_zero_point',
+                                        'weight_g_idx'),
+                 'gptq': ('qweight', 'qzeros', 'scales', 'g_idx')}
+
+    @classmethod
+    def _w4_unpack(cls, spec, t, name):
+        """one projection's checkpoint tensors {part: tensor} -> (u, s, z, group size) (ops' internal form)"""
+        if spec['format'] == 'gptq':
+            if 'qweight' not in t or 'qzeros' not in t or 'scales' not in t:
+                raise RuntimeError(f'checkpoint is missing GPTQ tensors of {name}: has {sorted(t)}')
+            out = ops.unpack_gptq_w4(t['qweight'], t['qzeros'], t['scales'], t.get('g_idx'))
+        else:
+            if 'weight_g_idx' in t:
+                raise ValueError(f'{name}.weight_g_idx: act-order compressed-tensors checkpoints are not supported')
+            if 'weight_packed' not in t or 'weight_scale' not in t or (not spec['sym'] and 'weight_zero_point' not in t):
+                raise RuntimeError(f'checkpoint is missing compressed-tensors tensors of {name}: has {sorted(t)}')
+            out = ops.unpack_compressed_tensors_w4(t['weight_packed'], t['weight_scale'], t.get('weight_shape'),
+                                                   t.get('weight_zero_point') if not spec['sym'] else None)
+        gs = spec['group_size'] or out[0].shape[1]
+        if out[3] != gs:
+            raise ValueError(f'{name}: the stored scales give group size {out[3]}, quantization_config says {gs}')
+        return out
+
+    def _install_w4_layer(self, layer, w):
+        """the layer's projections from {'q_proj': (u, s, z, gs), ...}: q|k|v and gate|up fused by rows (with their
+        scales and zero points), the HF names become Int4Rows views of the fused weights"""
+        a, m = layer.self_attn, layer.mlp
+        cat = lambda names, i: torch.cat([w[n][i] for n in names], dim=0).contiguous()
+        qkv_names = ('q_proj', 'k_proj', 'v_proj')
+        for names in (qkv_names, ('gate_proj', 'up_proj')):
+            if len({w[n][3] for n in names}) != 1:
+                raise ValueError(f'{"/".join(names)} have different group sizes: they cannot be fused')
+        nq, nk = w['q_proj'][0].shape[0], w['k_proj'][0].shape[0]
+        qkv = Int4Linear(cat(qkv_names, 0), cat(qkv_names, 1), cat(qkv_names, 2), w['q_proj'][3])
+        a.qkv_w4 = qkv
+        a.qkv_bias = None
+        if a.q_proj.bias is not None:
+            a.qkv_bias = torch.cat([a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data]).contiguous()
+        a.q_proj = Int4Rows(qkv, 0, nq, a.q_proj.bias)
+        a.k_proj = Int4Rows(qkv, nq, nq + nk, a.k_proj.bias)
+        a.v_proj = Int4Rows(qkv, nq + nk, qkv.shape[0], a.v_proj.bias)
+        a.qkv_weight = None
+        a.o_proj = Int4Linear(*w['o_proj'])
+        ni = w['gate_proj'][0].shape[0]
+        gu_names = ('gate_proj', 'up_proj')
+        gu = Int4Linear(cat(gu_names, 0), cat(gu_names, 1), cat(gu_names, 2), w['gate_proj'][3], interleaved=True)
+        m.gate_up_w4 = gu
+        m.gate_proj, m.up_proj = Int4Rows(gu, 0, ni), Int4Rows(gu, ni, 2 * ni)
+        m.gate_up_weight = None
+        m.down_proj = Int4Linear(*w['down_proj'])
+
+    @classmethod
+    @torch.no_grad()
+    def _from_pretrained_w4(cls, path, config, spec, device):
+        """As _from_pretrained_fp8: everything but the decoder projections is allocated up front; a layer's packed
+        tensors wait on the host until the layer is complete, then they are unpacked and tiled on the GPU, so no bf16
+        projection ever exists there."""
+        model, own, layer_of, _ = cls._fp8_skeleton(config, device)
+        dev = model.model.norm.weight.device
+        parts = cls._W4_PARTS[spec['format']]
+        need = {'qweight', 'qzeros', 'scales'} if spec['format'] == 'gptq' else \
+            {'weight_packed', 'weight_scale', 'weight_shape'} | (set() if spec['sym'] else {'weight_zero_point'})
+        pending = {li: {} for li in range(len(model.model.layers))}
+        seen = set()
+
+        def complete(li):
+            return all(need <= pending[li].get(f'model.layers.{li}.{p[:-len(".weight")]}', {}).keys()
+                       for p in cls._fp8_params)
+
+        def finish(li):
+            got = pending.pop(li)
+            w = {}
+            for p in cls._fp8_params:
+                name = f'model.layers.{li}.{p[:-len(".weight")]}'
+                w[p.rsplit('.', 2)[-2]] = cls._w4_unpack(spec, {k: v.to(dev) for k, v in got.get(name, {}).items()},
+                                                         name)
+            model._install_w4_layer(model.model.layers[li], w)
+
+        for sd in cls._shards(path):
+            for k, v in model._convert_checkpoint_keys(sd).items():
+                base, _, part = k.rpartition('.')
+                li = layer_of(base + '.weight') if part in parts else None
+                if li is not None and li in pending:
+                    pending[li].setdefault(base, {})[part] = v
+                elif part in parts and k.startswith(('lm_head.', 'model.embed_tokens.')):
+                    raise ValueError(f'{k}: a quantised {k.split(".")[0]} is not supported (it stays bf16)')
+                elif k in own:
+                    own[k].copy_(v.to(torch.bfloat16))
+                    seen.add(k)
+            # layers are finished at the end of a shard, so that an optional tensor (g_idx) stored after the required
+            # ones in the same shard is not missed
+            for li in [li for li in pending if complete(li)]:
+                finish(li)
+        if 'lm_head.weight' not in seen and getattr(config, 'tie_word_embeddings', False):
+            model.lm_head.weight.copy_(model.model.embed_tokens.weight)
+            seen.add('lm_head.weight')
+        missing = [k for k in own if k not in seen]
+        missing += [f'model.layers.{li}.* ({sorted(got)[:2]})' for li, got in pending.items()]
+        if missing:
+            raise RuntimeError(f'checkpoint is missing {len(missing)} tensors, e.g. {missing[:4]}')
+        model._fused = True
+        model._w4 = True
+        return model
+
+    @classmethod
+    @torch.no_grad()
+    def build_w4(cls, config, fill_rest, fill_codes, device=None):
+        """An int4 model without a checkpoint (synthetic weights, e.g. the benchmark's 70B shape): fill_rest(model)
+        initialises the parameters that stay bf16 (the projections are still meta tensors then); then, one layer at a
+        time, fill_codes(name, (N, K)) returns each projection's (u, s, z, group size) in ops' internal form on the
+        GPU (HF names, e.g. 'model.layers.3.self_attn.q_proj.weight')."""
+        model, _, _, _ = cls._fp8_skeleton(config, device)
+        fill_rest(model)
+        for li, layer in enumerate(model.model.layers):
+            w = {}
+            for p in cls._fp8_params:
+                mod = layer.get_submodule(p[:-len('.weight')])
+                w[p.rsplit('.', 2)[-2]] = fill_codes(f'model.layers.{li}.{p}', tuple(mod.weight.shape))
+            model._install_w4_layer(layer, w)
+        model._fused = True
+        model._w4 = True
+        return model
+
+    def _w4_plans(self, b):
+        """int4 GEMM plans of one activation buffer set, on the buffers (as _fp8_plans); the bf16 GEMM selection knobs
+        are refused"""
+        plans = getattr(b, 'w4_plans', None)
+        if plans is not None:
+            return plans
+        if os.environ.get('PIA_GEMM', '1') == '0' or 'PIA_GEMM_SET' in os.environ:
+            raise ValueError('this model holds int4 weights, which only the int4 GEMM runs: PIA_GEMM=0 / PIA_GEMM_SET '
+                             'do not apply')
+        b.fp8_out = torch.zeros((b.rows, self.config.hidden_size), dtype=torch.bfloat16, device=b.y.device)
+        if getattr(b, 'act', None) is None or b.act.shape[0] != b.rows:
+            b.act = torch.zeros((b.rows, self.config.intermediate_size), dtype=torch.bfloat16, device=b.y.device)
+        n_sm = torch.cuda.get_device_properties(b.y.device).multi_processor_count
+        plans = {'layers': []}
+        for layer in self.model.layers:
+            a, m = layer.self_attn, layer.mlp
+            bias = a.qkv_bias.float() if a.qkv_bias is not None else None
+            # the int4 GEMM's k chunk is 256 wide: _fp8_split's rule over chunks of that size
+            split = lambda w: self._fp8_split(torch.empty((w.shape[0], -(-w.shape[1] // 256) * 128), device='meta'), n_sm)
+            plans['layers'].append({
+                'qkv': a.qkv_w4.gemm(b.y, bias=bias, split_k=split(a.qkv_w4), out=b.qkv),
+                'o': a.o_proj.gemm(b.attn, split_k=split(a.o_proj), out=b.fp8_out),
+                'gate_up_silu': m.gate_up_w4.gemm(b.y, out=b.act).set_silu(),
+                'down': m.down_proj.gemm(b.act, split_k=split(m.down_proj), out=b.fp8_out)})
+        b.w4_plans = plans
+        return plans
+
     def _convert_checkpoint_keys(self, sd):
         """checkpoint tensor names -> this module tree's names (identity for Llama / Mistral)"""
         return sd
@@ -348,6 +627,9 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         both dimensions divisible by 128; otherwise ValueError before anything is converted."""
         if self._fp8:
             return self
+        if self._w4:
+            raise ValueError('quantize_fp8(): this model holds int4 weights from its checkpoint; they cannot be '
+                             're-quantised to fp8')
         self.fuse()
         for li, layer in enumerate(self.model.layers):
             for name, shape in self._fp8_weight_shapes(layer):
@@ -488,9 +770,10 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         plans = getattr(rt, 'gemm_plans', None)
         if plans is not None:
             return plans
-        if self._fp8:   # fp8 weights: the fp8 plans of both buffer sets instead, built here, outside any capture
-            self._fp8_plans(rt.decode_bufs)
-            self._fp8_plans(rt.prefill_bufs)
+        if self._fp8 or self._w4:   # fp8 / int4 weights: their plans of both buffer sets, built here, outside any capture
+            mk = self._fp8_plans if self._fp8 else self._w4_plans
+            mk(rt.decode_bufs)
+            mk(rt.prefill_bufs)
             rt.gemm_plans = False
             return False
         import os
@@ -638,9 +921,11 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         ops.embed_gather(self.model.embed_tokens.weight, b.ids, b.n_total, b.h)
         if self._fp8:   # every projection of every buffer set on the fp8 plans, over all rows of the buffers
             plans, rows = self._fp8_plans(b), b.rows
+        elif self._w4:  # likewise on the int4 plans
+            plans, rows = self._w4_plans(b), b.rows
         else:
             plans, rows = (self._gemm_plans(rt) if b is rt.decode_bufs else False), 64
-        pf = self._prefetch_cfg(rt) if plans and not self._fp8 else False
+        pf = self._prefetch_cfg(rt) if plans and not (self._fp8 or self._w4) else False
         fused_attn = b is rt.decode_bufs and os.environ.get('PIA_ATTN_FUSED', '0') != '0' and \
             (b.slots.batch == 1 or b.slots.kv_slot_stride != 0)
         if fused_attn:

@@ -55,6 +55,7 @@ class MixtralModel(LlamaModel):
 
 class MixtralForCausalLM(LlamaForCausalLM):
     model_cls = MixtralModel
+    int4_checkpoints = False   # no int4 weight mode for this family
     rmsnorm_rounding = ops.ROUND_TWICE   # weight * hidden_states.to(input_dtype) (mixtral/modeling_mixtral.py:165)
 
     def _fuse_mlp(self, layer):

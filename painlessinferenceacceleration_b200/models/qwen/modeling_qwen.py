@@ -108,6 +108,7 @@ def logn_table(seq_length, max_pos):
 class QWenLMHeadModel(LlamaForCausalLM):
     """module tree and parameter names are Llama's (checkpoint names are translated on load)"""
     model_cls = Qwen2Model   # the Llama decoder with biases on q / k / v
+    int4_checkpoints = False   # quantization_config is refused by the config check
     rmsnorm_rounding = ops.ROUND_ONCE   # (weight * (x * rsqrt(var + eps))).to(bf16): one rounding (:1262-1266)
 
     @staticmethod
