@@ -13,7 +13,9 @@
 //     X tile 64x64 (8 KB)} SWIZZLE_128B boxes.  ~100 KB of shared memory per CTA so that two CTAs share an SM and
 //     one CTA's prologue/epilogue hides behind the other's stream;
 //   * projections with few weight tiles (o_proj, down_proj: N = 4096 -> 32 tiles) split K across CTAs and write fp32
-//     partial slices that the consumer (k_rmsnorm_partials) sums in a fixed order - deterministic, no atomics.
+//     partial slices that the consumer (k_rmsnorm_partials) sums in a fixed order - deterministic, no atomics;
+//   * split-1 bf16 plans without an epilogue activation run k_gemm_stream instead: the same sums, 64- or 128-row tiles
+//     and one wgmma group in flight.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -330,6 +332,109 @@ k_gemm_ws(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
   }
 }
 
+// ------------------------------------------------------------------------------------------------ plain bf16 output
+// The split-1, non-cluster, non-SiLU plans (gate_up, lm_head): k_gemm_ws's accumulation - each output element summed
+// by one warpgroup over the full K, ascending 64-k chunks, 4 x wgmma m64n64k16 per chunk, one bf16 rounding - with
+//   * WG consumer warpgroups per CTA (a tile of 64 * WG weight rows);
+//   * one wgmma group kept in flight: the wgmmas of chunk i are issued before the group of chunk i - 1 is waited for,
+//     and only then is stage i - 1 released.  wgmmas on one accumulator complete in issue order, so the sum is the same.
+template <int WG, int NSTAGE>
+__global__ void __launch_bounds__(WG * 128 + 32, WG == 1 ? 3 : (NSTAGE <= 4 ? 2 : 1))
+k_gemm_stream(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, Params p) {
+  constexpr int TW_BYTES = WG * 64 * BK * 2, TSTAGE = TW_BYTES + X_BYTES, SMEM_BAR = NSTAGE * TSTAGE;
+  constexpr int NCW = WG * 4;  // consumer warps; the producer is warp NCW
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t bar_full = base + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE;
+  const int tile = blockIdx.x, nch = p.n_chunks;
+  const int n0 = tile * WG * 64;
+
+  if (tid == 0) {
+    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, NCW); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncwarp();
+  if (!p.no_pdl) pdl_launch_dependents();
+  __syncthreads();
+
+  if (warp == NCW) {
+    if (lane == 0) {
+      auto load_w = [&](int i, int s) {
+        const uint32_t wd = base + s * TSTAGE;
+        // tiled weight: [N/128][K/64] 16 KB blocks; with WG = 1 the map's boxes are their 8 KB halves of 64 rows
+        if (p.tiled) tma_load_3d(wd, &map_w, bar_full + 8 * s, 0, 0, WG == 2 ? tile * nch + i : 2 * ((tile >> 1) * nch + i) + (tile & 1));
+        else tma_load_2d(wd, &map_w, bar_full + 8 * s, i * BK, n0);
+      };
+      const int pre = nch < NSTAGE ? nch : NSTAGE;
+      for (int i = 0; i < pre; ++i) {
+        mbar_expect_tx(bar_full + 8 * i, TSTAGE);
+        load_w(i, i);
+      }
+      pdl_wait();
+      for (int i = 0; i < pre; ++i) tma_load_2d(base + i * TSTAGE + TW_BYTES, &map_x, bar_full + 8 * i, i * BK, 0);
+      for (int i = pre; i < nch; ++i) {
+        const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
+        mbar_wait(bar_empty + 8 * s, ph ^ 1);
+        mbar_expect_tx(bar_full + 8 * s, TSTAGE);
+        load_w(i, s);
+        tma_load_2d(base + s * TSTAGE + TW_BYTES, &map_x, bar_full + 8 * s, i * BK, 0);
+      }
+    }
+    return;
+  }
+
+  pdl_wait();
+  const int wg = warp >> 2;
+  float acc[32];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+  wgmma_fence();
+  for (int i = 0; i < nch; ++i) {
+    const int s = i % NSTAGE, ph = (i / NSTAGE) & 1;
+    mbar_wait(bar_full + 8 * s, ph);
+    const uint32_t wa = base + s * TSTAGE + wg * 64 * 128, xa = base + s * TSTAGE + TW_BYTES;
+#pragma unroll
+    for (int j = 0; j < BK / 16; ++j) wgmma_m64n64k16(acc, kmajor_desc(wa + j * 32), kmajor_desc(xa + j * 32));
+    wgmma_commit();
+    asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");  // chunk i - 1 is done with its stage
+    if (i > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * ((i - 1) % NSTAGE));
+    }
+  }
+  wgmma_wait_all();
+  fence_acc(acc);
+
+  // stage the tile [64 WG rows][64 tokens] through the dead pipeline stages; two threads per row, 32 tokens each
+  float *accs = reinterpret_cast<float *>(sm);
+  asm volatile("bar.sync 2, %0;" ::"n"(NCW * 32) : "memory");  // every consumer's wgmmas have read their last stage
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = wg * 64 + frag_row(warp, lane, h);
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<float2 *>(accs + r * ACC_LD + frag_tok(lane, i)) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+  }
+  asm volatile("bar.sync 2, %0;" ::"n"(NCW * 32) : "memory");
+  const int row = tid % (WG * 64), t0 = (tid / (WG * 64)) * 32;
+  const int n = n0 + row;
+  if (n < p.N) {
+    const float4 *src = reinterpret_cast<const float4 *>(accs + row * ACC_LD + t0);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const float4 a = src[q];
+      const int t = t0 + 4 * q;
+      if (t < p.rows) p.out_bf16[(long long)t * p.N + n] = __float2bfloat16_rn(a.x);
+      if (t + 1 < p.rows) p.out_bf16[(long long)(t + 1) * p.N + n] = __float2bfloat16_rn(a.y);
+      if (t + 2 < p.rows) p.out_bf16[(long long)(t + 2) * p.N + n] = __float2bfloat16_rn(a.z);
+      if (t + 3 < p.rows) p.out_bf16[(long long)(t + 3) * p.N + n] = __float2bfloat16_rn(a.w);
+    }
+  }
+}
+template <int WG, int NSTAGE>
+constexpr int stream_smem_total() { return NSTAGE * (WG * 64 * BK * 2 + X_BYTES) + 16 * NSTAGE + 1024; }
 
 // ------------------------------------------------------------------------------------------------ stream-K
 // Work = n_tiles x n_chunks (tile, k-chunk) units, cut into gridDim.x equal contiguous ranges: every SM streams
@@ -1012,8 +1117,10 @@ using namespace pia::gemm;
 
 struct pia_gemm_plan {
   CUtensorMap map_w, map_x;
+  CUtensorMap map_w64;  // the weight in 64-row boxes (k_gemm_stream with one consumer warpgroup)
   Params p;
   int nstage;
+  int stream_wg;        // consumer warpgroups (64-row slices) per tile of the split-1 bf16 kernel k_gemm_stream
   int no_pdl;  // 1: launched without the programmatic-dependent-launch attribute (a plain kernel boundary, like cuBLAS)
   // stream-K mode
   int stream_k, sk_grid;
@@ -1049,6 +1156,21 @@ static int encode_tiled_w(CUtensorMap *m, const void *base, uint64_t n_blocks) {
   cuuint64_t dims[3] = {(cuuint64_t)BK, (cuuint64_t)BMW, n_blocks};
   cuuint64_t strides[2] = {(cuuint64_t)BK * 2, (cuuint64_t)BK * BMW * 2};
   cuuint32_t box[3] = {BK, BMW, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return PIA_ERR_CUDA; }
+  return PIA_OK;
+}
+
+// the same tiled weight as 8 KB boxes of 64 rows x 64 k: box 2b + h is half h of block b
+static int encode_tiled_w64(CUtensorMap *m, const void *base, uint64_t n_blocks) {
+  EncodeTiledFn fn = get_encode();
+  PIA_REQUIRE(fn, "cuTensorMapEncodeTiled not available in this driver");
+  cuuint64_t dims[3] = {(cuuint64_t)BK, 64, 2 * n_blocks};
+  cuuint64_t strides[2] = {(cuuint64_t)BK * 2, (cuuint64_t)BK * 64 * 2};
+  cuuint32_t box[3] = {BK, 64, 1};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(base), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1113,10 +1235,19 @@ extern "C" int pia_gemm_plan_create(const void *d_w, int N, int K, const void *d
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     const int ctas = ((N + BMW - 1) / BMW) * g->p.n_split;
     g->nstage = ctas <= n_sm ? 8 : 4;
+    // split-1 bf16 plans: 64-row tiles when they fit in one wave at 3 CTAs per SM (gate_up: 344 tiles on 132 SMs),
+    // which evens out the bytes each SM streams; else 128-row tiles (lm_head: 500 64-row tiles would need a second
+    // wave).  Measured on gate_up: 64.0 us vs 69.8 us with 128-row tiles; lm_head: 94.0 us vs 88.2 us (DESIGN.md 9)
+    g->stream_wg = (N + 63) / 64 <= 3 * n_sm ? 1 : 2;
     cudaError_t e = cudaFuncSetAttribute(k_gemm_ws<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_total(4));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_ws<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_total(8));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_stream<2, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_total<2, 4>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_stream<2, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_total<2, 8>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_stream<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_total<1, 4>());
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); rc = PIA_ERR_CUDA; }
   }
+  if (rc == PIA_OK) rc = w_tiled ? encode_tiled_w64(&g->map_w64, d_w, (uint64_t)(N / BMW) * n_chunks)
+                                 : encode_2d(&g->map_w64, d_w, (uint64_t)K, (uint64_t)N, BK, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   g->stream_k = 0; g->no_pdl = 0;
   if (rc == PIA_OK && want_stream_k) {
     // stream-K over the HBM-tiled weight: grid = min(#SMs, units), fix-up workspace owned by the plan
@@ -1414,6 +1545,17 @@ extern "C" int pia_gemm_run(pia_gemm_plan_t *g, int rows, void *d_out, void *str
     dim3 cgrid(p.n_split, (p.N + BMW - 1) / BMW);
     if (g->nstage == 8) PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_ws<8>, cgrid, dim3(NTHREADS), smem_total(8), (cudaStream_t)stream, (unsigned)p.cluster, g->map_w, g->map_x, p));
     else PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_ws<4>, cgrid, dim3(NTHREADS), smem_total(4), (cudaStream_t)stream, (unsigned)p.cluster, g->map_w, g->map_x, p));
+    count_launch();
+    return PIA_OK;
+  }
+  if (p.n_split == 1 && !p.silu && p.groups == 1) {
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (g->stream_wg == 1)
+      PIA_CUDA_CHECK(launch_kernel(k_gemm_stream<1, 4>, dim3((p.N + 63) / 64), dim3(160), stream_smem_total<1, 4>(), st, g->map_w64, g->map_x, p));
+    else if (g->nstage == 8)
+      PIA_CUDA_CHECK(launch_kernel(k_gemm_stream<2, 8>, dim3((p.N + BMW - 1) / BMW), dim3(NTHREADS), stream_smem_total<2, 8>(), st, g->map_w, g->map_x, p));
+    else
+      PIA_CUDA_CHECK(launch_kernel(k_gemm_stream<2, 4>, dim3((p.N + BMW - 1) / BMW), dim3(NTHREADS), stream_smem_total<2, 4>(), st, g->map_w, g->map_x, p));
     count_launch();
     return PIA_OK;
   }

@@ -839,42 +839,6 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             return ops.Gemm(cache[key], x, split_k=split_k, tiled=True)
         return ops.Gemm(w.contiguous(), x, split_k=split_k)
 
-    # ------------------------------------------------------------------ weight prefetch beside the small kernels
-    def _prefetch_cfg(self, rt):
-        """PIA_PREFETCH="o_frac,gate_up_frac,down_frac,gbytes_per_s" (0 disables): which share of the next
-        projections' weights is pulled into L2 on a side stream while RoPE + tree attention (o, gate_up) and
-        SiLU*up (down) keep HBM idle; the step is weight-streaming bound, so HBM time hidden here comes straight
-        off the step.  Decode steps only."""
-        cfg = getattr(rt, 'prefetch_cfg', None)
-        if cfg is None:
-            import os
-            spec = os.environ.get('PIA_PREFETCH', '0')
-            v = [float(t) for t in spec.split(',')] if spec not in ('', '0') else []
-            cfg = False
-            if v and torch.cuda.is_available():
-                v = (v + [0.0] * 4)[:4]
-                cfg = dict(o=v[0], gate_up=v[1], down=v[2], rate=v[3], side=torch.cuda.Stream(device=self.device))
-            rt.prefetch_cfg = cfg
-        return cfg
-
-    @staticmethod
-    def _prefetch(pf, jobs):
-        """fork: the side stream picks up after the kernels launched so far and issues the prefetch jobs"""
-        main = torch.cuda.current_stream()
-        pf['side'].wait_stream(main)
-        with torch.cuda.stream(pf['side']):
-            for (t, frac, tile_bytes) in jobs:
-                if frac <= 0:
-                    continue
-                total = t.numel() * t.element_size()
-                if tile_bytes:   # HBM-tiled weight: the first share of every tile (= its first k chunks)
-                    rb = max(16384, int(tile_bytes * min(frac, 1.0)) // 16384 * 16384)
-                    ops.l2_prefetch(t, n_ranges=total // tile_bytes, stride_bytes=tile_bytes, range_bytes=min(rb, tile_bytes),
-                                    gbytes_per_s=pf['rate'])
-                else:
-                    ops.l2_prefetch(t, range_bytes=int(total * min(frac, 1.0)) // 16 * 16, gbytes_per_s=pf['rate'])
-        pf['dirty'] = True
-
     def _check_fused_attn(self):
         """the fused RoPE-inside-attention kernel (PIA_ATTN_FUSED) rotates in the half-split layout only"""
         if self.rotary_interleaved and os.environ.get('PIA_ATTN_FUSED', '0') != '0':
@@ -882,7 +846,7 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                              'kernel does not: unset PIA_ATTN_FUSED')
 
     # ------------------------------------------------------------------ the verify forward on static buffers
-    def _mlp(self, rt, layer, y, plans=None, pf=None, b=None):
+    def _mlp(self, rt, layer, y, plans=None, b=None):
         """returns (x, parts): the MLP output as a bf16 tensor or as fp32 split-K slices for the next rmsnorm.
         b: the buffer set y belongs to (default: the decode buffers)"""
         m = layer.mlp
@@ -896,8 +860,6 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                     plans['gate_up'].run(64, out=b.gu)
                 else:
                     torch.mm(y, m.gate_up_weight.t(), out=b.gu)
-                if pf:
-                    self._prefetch(pf, [(m.down_proj.weight, pf['down'], 0)])
                 ops.silu_mul(b.gu, b.act)
             if 'down' in plans:
                 o = plans['down'].run(rows)
@@ -925,7 +887,6 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             plans, rows = self._w4_plans(b), b.rows
         else:
             plans, rows = (self._gemm_plans(rt) if b is rt.decode_bufs else False), 64
-        pf = self._prefetch_cfg(rt) if plans and not (self._fp8 or self._w4) else False
         fused_attn = b is rt.decode_bufs and os.environ.get('PIA_ATTN_FUSED', '0') != '0' and \
             (b.slots.batch == 1 or b.slots.kv_slot_stride != 0)
         if fused_attn:
@@ -960,10 +921,6 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
                 torch.addmm(a.qkv_bias, b.y, a.qkv_weight.t(), out=b.qkv)
             else:
                 torch.mm(b.y, a.qkv_weight.t(), out=b.qkv)
-            if pf and lp and 'gate_up' in lp:
-                gw = lp['gate_up'].weight
-                self._prefetch(pf, [(a.o_proj.weight, pf['o'], 0),
-                                    (gw, pf['gate_up'], gw.shape[1] * gw.shape[2] * gw.shape[3] * 2 if gw.dim() == 4 else 0)])
             # every request slot / prefill chunk of the table in one launch each (pia_slots_t)
             if fused_attn:   # decode steps: RoPE + KV append happen inside the attention kernel
                 rt.plan.forward_fused(li, b.qkv, b.mask, b.slots, rt.rope_cos, rt.rope_sin, b.attn)
@@ -980,11 +937,9 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             if self.sandwich_norms:
                 x, parts = post_norm(layer.post_self_attn_layernorm.weight)
             norm(layer.post_attention_layernorm.weight)
-            x, parts = self._mlp(rt, layer, b.y, lp, pf, b=b)
+            x, parts = self._mlp(rt, layer, b.y, lp, b=b)
             if self.sandwich_norms:
                 x, parts = post_norm(layer.post_mlp_layernorm.weight)
-        if pf and pf.pop('dirty', False):  # join the side stream (required before a capture ends)
-            torch.cuda.current_stream().wait_stream(pf['side'])
         if last_only:
             return
         norm(self.model.norm.weight)

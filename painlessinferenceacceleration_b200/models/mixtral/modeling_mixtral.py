@@ -153,7 +153,7 @@ class MixtralForCausalLM(LlamaForCausalLM):
         plans['moe_down'] = ops.Gemm.grouped_fp8(ex.down_proj.qweight, ex.down_proj.scale, b.moe_act)
         return plans
 
-    def _mlp(self, rt, layer, y, plans=None, pf=None, b=None):
+    def _mlp(self, rt, layer, y, plans=None, b=None):
         moe = layer.mlp
         if plans:
             b = b if b is not None else rt.decode_bufs

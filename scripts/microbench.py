@@ -57,7 +57,7 @@ def timeit(name, fn, per, reps=20, bytes_per=None):
 NL = g['n_layers']
 layers = model.model.layers
 if a.forward_only:
-    timeit('verify layers (whole forward) PIA_PREFETCH=' + os.environ.get('PIA_PREFETCH', '0'), lambda: model._verify_layers(rt), 1,
+    timeit('verify layers (whole forward)', lambda: model._verify_layers(rt), 1,
            bytes_per=sum(p.numel() for p in model.parameters()) * 2)
     sys.exit(0)
 L = a.P + a.n
