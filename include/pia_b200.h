@@ -294,6 +294,15 @@ int pia_gemm_plan_create_grouped_fp8(const void *d_w, const void *d_scale, int g
 int pia_gemm_plan_create_w4(const void *d_codes, const void *d_scale, const void *d_zero, int scale_dtype,
                             const void *d_bias, int N, int K, int group_size, const void *d_x, int x_rows, int split_k,
                             pia_gemm_plan_t **out);
+/* Grouped int4 twin (MoE experts): `groups` weights [N, K] stacked by rows to one [groups * N, K] weight, tiled by
+ * ops.tile_weight_w4 as one matrix; d_scale / d_zero [K/group, groups * N] (the stacked rows' tables, group g's
+ * columns start at g * N).  out[g] ([x_rows, N] bf16, consecutive) = X[:, g*K : (g+1)*K] @ W[g]^T for 1 <= rows <=
+ * x_rows.  One K split, no bias; set_silu and set_relu are refused.  PIA_ERR_INVALID, launching nothing, for
+ * groups < 1, N or K not a multiple of 128, a group size that is not a multiple of 128 dividing K, misaligned operands
+ * or x_rows < 64. */
+int pia_gemm_plan_create_grouped_w4(const void *d_codes, const void *d_scale, const void *d_zero, int scale_dtype,
+                                    int groups, int N, int K, int group_size, const void *d_x, int x_rows,
+                                    pia_gemm_plan_t **out);
 
 /* ============================================================================================
  * Fused elementwise pieces of the verify forward (all bf16 I/O, fp32 math)

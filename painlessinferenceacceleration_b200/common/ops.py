@@ -324,6 +324,30 @@ class Gemm(object):
         self.out = torch.empty((G, x.shape[0], N), dtype=torch.bfloat16, device=x.device)
         return self
 
+    @classmethod
+    def grouped_w4(cls, codes, scale_t, zero_t, group_size, groups, x):
+        """one int4 launch for all experts (pia_gemm_plan_create_grouped_w4): codes = tile_weight_w4 of the [G * N, K]
+        row stack of G weights, scale_t / zero_t [K/group, G * N] (the stack's tables), x [rows, G * K]; runs
+        1..x.shape[0] rows; out bf16 [G, x_rows, N]"""
+        ng, GN = scale_t.shape
+        K, G = ng * group_size, int(groups)
+        N = GN // G
+        assert G >= 1 and N * G == GN
+        assert codes.dtype == torch.uint8 and codes.is_contiguous() and tuple(codes.shape) == (GN // 128, -(-K // 256), 128, 128)
+        assert scale_t.dtype in W4_SCALE_DTYPES and scale_t.is_contiguous()
+        assert zero_t.dtype == torch.uint8 and tuple(zero_t.shape) == (ng, GN) and zero_t.is_contiguous()
+        assert x.shape[1] == G * K and x.is_contiguous()
+        self = cls.__new__(cls)
+        self.lib = L.load()
+        self.h = L.vp()
+        with torch.cuda.device(codes.device):
+            L.check(self.lib.pia_gemm_plan_create_grouped_w4(_p(codes), _p(scale_t), _p(zero_t),
+                                                             int(scale_t.dtype == torch.float16), G, N, K,
+                                                             int(group_size), _p(x), x.shape[0], C.byref(self.h)))
+        self.splits, self.N, self.weight, self._keep = 1, N, codes, (codes, scale_t, zero_t, x)
+        self.out = torch.empty((G, x.shape[0], N), dtype=torch.bfloat16, device=x.device)
+        return self
+
     def set_pdl(self, on=True):
         L.check(self.lib.pia_gemm_plan_set_pdl(self.h, int(on)))
         return self

@@ -860,6 +860,10 @@ struct W4Params {
   const float *bias;           // [N] or null
   __nv_bfloat16 *out_bf16;
   float *out_f32;
+  // grouped (MoE experts; k_gemm_w4<.., GROUPED = true> only): `groups` stacked [N, K] weights, the tables [K / group,
+  // groups * N], X [x_rows, groups * K]; group g's output [x_rows, N] starts out_group_stride elements after g - 1's
+  int groups;
+  long long out_group_stride;
 };
 
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
@@ -882,8 +886,10 @@ __device__ __forceinline__ uint32_t w4_deq(uint32_t w, uint32_t zo, uint32_t sc)
 }
 
 // NSTAGE = 2: ~107 KB of shared memory, two CTAs per SM; NSTAGE = 4: ~205 KB, one CTA per SM (grids that do not fill
-// the SMs twice) - 64 KB of code bytes (128 K weights) in flight per SM either way
-template <int NSTAGE, bool F16>
+// the SMs twice) - 64 KB of code bytes (128 K weights) in flight per SM either way.
+// GROUPED: gridDim.z = groups x 64-row token blocks; group g = one MoE expert reads code blocks of tiles [g * tiles,
+// +tiles), table columns [g * N, +N) and X columns [g * K, +K), and writes out[g].  One K split, no bias, no SiLU.
+template <int NSTAGE, bool F16, bool GROUPED = false>
 __global__ void __launch_bounds__(NTHREADS, NSTAGE <= 2 ? 2 : 1)
 k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, W4Params p) {
   constexpr int SMEM_BAR = NSTAGE * W4_STAGE_BYTES;
@@ -894,7 +900,8 @@ k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
   const uint32_t bar_full = base + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE;
   const int tile = p.cluster ? blockIdx.y : blockIdx.x, split = p.cluster ? blockIdx.x : blockIdx.y;
   const int n0 = tile * BMW;
-  const int t0 = blockIdx.z * TOK;  // first token row of this CTA
+  int grp = 0, t0 = blockIdx.z * TOK;  // group, first token row of this CTA
+  if (GROUPED) { grp = blockIdx.z / p.ntb; t0 = (blockIdx.z % p.ntb) * TOK; }
   const int rows = p.rows - t0 < TOK ? p.rows - t0 : TOK;
   const int c0 = split * p.chunks_per_split;
   int c1 = c0 + p.chunks_per_split;
@@ -913,8 +920,12 @@ k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
   if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       // codes, scales and zero points are immutable: the first NSTAGE stages stream before griddepcontrol.wait
-      const int wblk = tile * p.n_chunks + c0;
+      const int wblk = ((GROUPED ? grp * p.tiles : 0) + tile) * p.n_chunks + c0;
+      const int xb0 = GROUPED ? grp * (p.K / BK) : 0;                      // X: the group's first 64-k box
       constexpr int sb = 2;  // bytes per scale (bf16 or fp16)
+      // entry (g, n0) of a [K / group, N] table; grouped: the tables are groups * N wide, this group's columns start
+      // at grp * N
+      auto meta = [&](long long g) { return GROUPED ? g * p.groups * p.N + grp * p.N + n0 : g * p.N + n0; };
       auto halves = [&](int i) { return 2 * (c0 + i) + 1 < khalves ? 2 : 1; };
       auto stage_bytes = [&](int i) { return (uint32_t)(W4_W_BYTES + halves(i) * (2 * X_BYTES + BMW * (sb + 1))); };
       auto load_w = [&](int i, int s) {
@@ -923,13 +934,13 @@ k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
         for (int h = 0; h < halves(i); ++h) {
           const long long g = (long long)((c0 + i) * W4_BK + h * 128) / p.group;
           bulk_load(st + W4_META_OFF + h * BMW * sb,
-                    reinterpret_cast<const uint8_t *>(p.scale) + (g * p.N + n0) * sb, BMW * sb, bar);
-          bulk_load(st + W4_META_OFF + 2 * BMW * sb + h * BMW, p.zero + g * p.N + n0, BMW, bar);
+                    reinterpret_cast<const uint8_t *>(p.scale) + meta(g) * sb, BMW * sb, bar);
+          bulk_load(st + W4_META_OFF + 2 * BMW * sb + h * BMW, p.zero + meta(g), BMW, bar);
         }
       };
       auto load_x = [&](int i, int s) {
         const uint32_t xd = base + s * W4_STAGE_BYTES + W4_X_OFF;
-        for (int b = 0; b < 2 * halves(i); ++b) tma_load_2d(xd + b * X_BYTES, &map_x, bar_full + 8 * s, ((c0 + i) * 4 + b) * BK, t0);
+        for (int b = 0; b < 2 * halves(i); ++b) tma_load_2d(xd + b * X_BYTES, &map_x, bar_full + 8 * s, (xb0 + (c0 + i) * 4 + b) * BK, t0);
       };
       const int pre = nch < NSTAGE ? nch : NSTAGE;
       for (int i = 0; i < pre; ++i) {
@@ -947,7 +958,7 @@ k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
       }
     }
     __syncwarp();
-    if (p.cluster) { cluster_sync_all(); cluster_sync_all(); }
+    if (!GROUPED && p.cluster) { cluster_sync_all(); cluster_sync_all(); }
     return;
   }
 
@@ -1017,7 +1028,7 @@ k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
   }
   asm volatile("bar.sync 2, 256;" ::: "memory");
   if (wg == 1) {
-    if (p.cluster) { cluster_sync_all(); cluster_sync_all(); }
+    if (!GROUPED && p.cluster) { cluster_sync_all(); cluster_sync_all(); }
     return;
   }
 
@@ -1033,7 +1044,7 @@ k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
       v[4 * t] = a.x; v[4 * t + 1] = a.y; v[4 * t + 2] = a.z; v[4 * t + 3] = a.w;
     }
   }
-  if (p.cluster) {
+  if (!GROUPED && p.cluster) {
     const int cs = p.cluster, RS = BMW / cs;
     cluster_sync_all();
     {
@@ -1065,7 +1076,7 @@ k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
         if (tt + 3 < rows) ob[(long long)(tt + 3) * p.N + n_out] = __float2bfloat16_rn(a.w);
       }
     }
-  } else if (p.silu) {
+  } else if (!GROUPED && p.silu) {
     __nv_bfloat16 *xu = reinterpret_cast<__nv_bfloat16 *>(sm + SMEM_BAR + 256);
     __nv_bfloat16 *xg = xu + 32 * 64;
     const int rr = (q & 1) * 32 + lane;
@@ -1090,14 +1101,14 @@ k_gemm_w4(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUt
         ob[(long long)(tb + t) * inter + col] = __float2bfloat16_rn(sg * u);
       }
     }
-  } else if (p.n_split == 1) {
+  } else if (GROUPED || p.n_split == 1) {
     // no bias: the accumulator is rounded as it is (k_gemm_ws's epilogue; + 0.f would turn a -0 into +0)
-    if (p.bias) {
+    if (!GROUPED && p.bias) {
       const float bs = p.bias[n];
 #pragma unroll
       for (int t = 0; t < TOK; ++t) v[t] += bs;
     }
-    __nv_bfloat16 *ob = p.out_bf16 + (long long)t0 * p.N;
+    __nv_bfloat16 *ob = p.out_bf16 + (GROUPED ? grp * p.out_group_stride : 0) + (long long)t0 * p.N;
 #pragma unroll
     for (int t = 0; t < TOK; ++t)
       if (t < rows) ob[(long long)t * p.N + n] = __float2bfloat16_rn(v[t]);
@@ -1128,8 +1139,8 @@ struct pia_gemm_plan {
   // fp8 weight mode (pia_gemm_plan_create_fp8 / _grouped_fp8): k_gemm_fp8 with `f`, up to x_rows rows per run
   int fp8, groups, x_rows;
   F8Params f;
-  // int4 weight mode (pia_gemm_plan_create_w4): k_gemm_w4 with `w`, up to x_rows rows per run
-  int w4, w4_f16;
+  // int4 weight mode (pia_gemm_plan_create_w4 / _grouped_w4): k_gemm_w4 with `w`, up to x_rows rows per run
+  int w4, w4_f16, w4_grouped;
   W4Params w;
 };
 
@@ -1308,6 +1319,7 @@ extern "C" int pia_gemm_plan_set_silu(pia_gemm_plan_t *g, int on) {
     return PIA_OK;
   }
   if (g && g->w4) {
+    PIA_REQUIRE(!g->w4_grouped, "the SiLU*up epilogue needs one group: a grouped int4 plan has none");
     PIA_REQUIRE(g->w.n_split == 1 && !g->w.bias, "the SiLU*up epilogue needs split_k == 1 and no bias");
     g->w.silu = on ? 1 : 0;
     return PIA_OK;
@@ -1431,11 +1443,15 @@ extern "C" int pia_gemm_plan_create_grouped_fp8(const void *d_w, const void *d_s
 }
 
 // int4 codes, tiled by ops.tile_weight_w4: [N/128][ceil(K/256)] contiguous 16 KB blocks of 128 rows x 128 bytes (256
-// nibbles), one SWIZZLE_128B TMA box each
+// nibbles), one SWIZZLE_128B TMA box each.  groups > 0: a grouped plan (groups stacked weights, one K split, no bias)
 static int w4_plan_create(const void *d_codes, const void *d_scale, const void *d_zero, int scale_f16,
-                          const void *d_bias, int N, int K, int group, const void *d_x, int x_rows, int split_k,
-                          pia_gemm_plan_t **out) {
+                          const void *d_bias, int groups, int N, int K, int group, const void *d_x, int x_rows,
+                          int split_k, pia_gemm_plan_t **out) {
   PIA_REQUIRE(d_codes && d_scale && d_zero && d_x && out, "null argument");
+  const int grouped = groups > 0;
+  if (!grouped) groups = 1;
+  PIA_REQUIRE(groups >= 1 && groups <= 4096, "groups %d outside [1, 4096]", groups);
+  PIA_REQUIRE(!grouped || (split_k == 1 && !d_bias), "a grouped int4 plan has one K split and no bias");
   PIA_REQUIRE(N > 0 && N % BMW == 0 && K > 0 && K % 128 == 0, "the int4 GEMM needs N %% %d == 0 and K %% 128 == 0", BMW);
   PIA_REQUIRE(group > 0 && group % 128 == 0 && K % group == 0, "group size %d: a multiple of 128 that divides K = %d", group, K);
   PIA_REQUIRE(scale_f16 == 0 || scale_f16 == 1, "scale dtype: 0 = bf16, 1 = fp16");
@@ -1457,23 +1473,29 @@ static int w4_plan_create(const void *d_codes, const void *d_scale, const void *
   w.cluster = 0; w.silu = 0; w.no_pdl = 0;
   w.scale = d_scale; w.zero = (const uint8_t *)d_zero; w.bias = (const float *)d_bias;
   w.out_bf16 = nullptr; w.out_f32 = nullptr;
+  w.groups = groups; w.out_group_stride = (long long)x_rows * N;
   if (want_cluster && w.n_split != want_cluster) { set_error("K = %d is too short for %d cluster splits", K, want_cluster); return PIA_ERR_INVALID; }
   w.cluster = want_cluster;
   if (d_bias && w.n_split > 1 && !w.cluster) { set_error("a bias needs split_k == 1 or a cluster split"); return PIA_ERR_INVALID; }
   pia_gemm_plan *g = new (std::nothrow) pia_gemm_plan();
   PIA_REQUIRE(g, "out of host memory");
-  g->w = w; g->w4 = 1; g->w4_f16 = scale_f16; g->groups = 1; g->x_rows = x_rows;
-  int rc = encode_tiled_w_fp8(&g->map_w, d_codes, (uint64_t)w.tiles * n_chunks);   // the same 128 x 128-byte boxes
-  if (rc == PIA_OK) rc = encode_2d(&g->map_x, d_x, (uint64_t)K, (uint64_t)x_rows, BK, TOK, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  g->w = w; g->w4 = 1; g->w4_f16 = scale_f16; g->w4_grouped = grouped; g->groups = groups; g->x_rows = x_rows;
+  // the same 128 x 128-byte boxes
+  int rc = encode_tiled_w_fp8(&g->map_w, d_codes, (uint64_t)groups * w.tiles * n_chunks);
+  if (rc == PIA_OK) rc = encode_2d(&g->map_x, d_x, (uint64_t)groups * K, (uint64_t)x_rows, BK, TOK, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc == PIA_OK) {
     int n_sm = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    g->nstage = w.tiles * w.n_split <= n_sm ? 4 : 2;
+    g->nstage = w.tiles * w.n_split * groups <= n_sm ? 4 : 2;
     cudaError_t e = cudaFuncSetAttribute(k_gemm_w4<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(2));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(4));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(2));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(4));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(2));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<4, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(4));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<2, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(2));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_w4<4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, w4_smem_total(4));
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); rc = PIA_ERR_CUDA; }
   }
   if (rc != PIA_OK) { delete g; return rc; }
@@ -1484,7 +1506,14 @@ static int w4_plan_create(const void *d_codes, const void *d_scale, const void *
 extern "C" int pia_gemm_plan_create_w4(const void *d_codes, const void *d_scale, const void *d_zero, int scale_dtype,
                                        const void *d_bias, int N, int K, int group_size, const void *d_x, int x_rows,
                                        int split_k, pia_gemm_plan_t **out) {
-  return w4_plan_create(d_codes, d_scale, d_zero, scale_dtype, d_bias, N, K, group_size, d_x, x_rows, split_k, out);
+  return w4_plan_create(d_codes, d_scale, d_zero, scale_dtype, d_bias, 0, N, K, group_size, d_x, x_rows, split_k, out);
+}
+
+extern "C" int pia_gemm_plan_create_grouped_w4(const void *d_codes, const void *d_scale, const void *d_zero,
+                                               int scale_dtype, int groups, int N, int K, int group_size,
+                                               const void *d_x, int x_rows, pia_gemm_plan_t **out) {
+  PIA_REQUIRE(groups >= 1, "groups %d: a grouped int4 plan needs at least one group", groups);
+  return w4_plan_create(d_codes, d_scale, d_zero, scale_dtype, nullptr, groups, N, K, group_size, d_x, x_rows, 1, out);
 }
 
 struct PdlScope { int on; explicit PdlScope(int off) : on(off) { if (on) ++pia::g_pdl_off; } ~PdlScope() { if (on) --pia::g_pdl_off; } };
@@ -1513,7 +1542,17 @@ static int w4_run(pia_gemm_plan_t *g, int rows, void *d_out, void *stream) {
   const dim3 grid = w.cluster ? dim3(w.n_split, w.tiles, w.ntb) : dim3(w.tiles, w.n_split, w.ntb);
   const unsigned cs = w.cluster ? (unsigned)w.cluster : 1u;
   const cudaStream_t st = (cudaStream_t)stream;
-  if (g->nstage == 4) {
+  if (g->w4_grouped) {
+    PIA_REQUIRE((long long)g->groups * w.ntb <= 65535, "%d groups x %d token blocks exceed gridDim.z", g->groups, w.ntb);
+    const dim3 gg(w.tiles, 1, (unsigned)(g->groups * w.ntb));
+    if (g->nstage == 4) {
+      if (g->w4_f16) PIA_CUDA_CHECK(launch_kernel(k_gemm_w4<4, true, true>, gg, dim3(NTHREADS), w4_smem_total(4), st, g->map_w, g->map_x, w));
+      else PIA_CUDA_CHECK(launch_kernel(k_gemm_w4<4, false, true>, gg, dim3(NTHREADS), w4_smem_total(4), st, g->map_w, g->map_x, w));
+    } else {
+      if (g->w4_f16) PIA_CUDA_CHECK(launch_kernel(k_gemm_w4<2, true, true>, gg, dim3(NTHREADS), w4_smem_total(2), st, g->map_w, g->map_x, w));
+      else PIA_CUDA_CHECK(launch_kernel(k_gemm_w4<2, false, true>, gg, dim3(NTHREADS), w4_smem_total(2), st, g->map_w, g->map_x, w));
+    }
+  } else if (g->nstage == 4) {
     if (g->w4_f16) PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_w4<4, true>, grid, dim3(NTHREADS), w4_smem_total(4), st, cs, g->map_w, g->map_x, w));
     else PIA_CUDA_CHECK(launch_kernel_cluster(k_gemm_w4<4, false>, grid, dim3(NTHREADS), w4_smem_total(4), st, cs, g->map_w, g->map_x, w));
   } else {

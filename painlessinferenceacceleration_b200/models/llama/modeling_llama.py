@@ -455,12 +455,27 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
     def _install_w4_layer(self, layer, w):
         """the layer's projections from {'q_proj': (u, s, z, gs), ...}: q|k|v and gate|up fused by rows (with their
         scales and zero points), the HF names become Int4Rows views of the fused weights"""
-        a, m = layer.self_attn, layer.mlp
+        m = layer.mlp
+        cat = lambda names, i: torch.cat([w[n][i] for n in names], dim=0).contiguous()
+        if w['gate_proj'][3] != w['up_proj'][3]:
+            raise ValueError('gate_proj/up_proj have different group sizes: they cannot be fused')
+        self._install_w4_attn(layer, w)
+        ni = w['gate_proj'][0].shape[0]
+        gu_names = ('gate_proj', 'up_proj')
+        gu = Int4Linear(cat(gu_names, 0), cat(gu_names, 1), cat(gu_names, 2), w['gate_proj'][3], interleaved=True)
+        m.gate_up_w4 = gu
+        m.gate_proj, m.up_proj = Int4Rows(gu, 0, ni), Int4Rows(gu, ni, 2 * ni)
+        m.gate_up_weight = None
+        m.down_proj = Int4Linear(*w['down_proj'])
+
+    def _install_w4_attn(self, layer, w):
+        """q|k|v fused by rows (with their scales and zero points; the HF names become Int4Rows views) and o_proj, from
+        {'q_proj': (u, s, z, gs), ...}"""
+        a = layer.self_attn
         cat = lambda names, i: torch.cat([w[n][i] for n in names], dim=0).contiguous()
         qkv_names = ('q_proj', 'k_proj', 'v_proj')
-        for names in (qkv_names, ('gate_proj', 'up_proj')):
-            if len({w[n][3] for n in names}) != 1:
-                raise ValueError(f'{"/".join(names)} have different group sizes: they cannot be fused')
+        if len({w[n][3] for n in qkv_names}) != 1:
+            raise ValueError(f'{"/".join(qkv_names)} have different group sizes: they cannot be fused')
         nq, nk = w['q_proj'][0].shape[0], w['k_proj'][0].shape[0]
         qkv = Int4Linear(cat(qkv_names, 0), cat(qkv_names, 1), cat(qkv_names, 2), w['q_proj'][3])
         a.qkv_w4 = qkv
@@ -472,13 +487,6 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
         a.v_proj = Int4Rows(qkv, nq + nk, qkv.shape[0], a.v_proj.bias)
         a.qkv_weight = None
         a.o_proj = Int4Linear(*w['o_proj'])
-        ni = w['gate_proj'][0].shape[0]
-        gu_names = ('gate_proj', 'up_proj')
-        gu = Int4Linear(cat(gu_names, 0), cat(gu_names, 1), cat(gu_names, 2), w['gate_proj'][3], interleaved=True)
-        m.gate_up_w4 = gu
-        m.gate_proj, m.up_proj = Int4Rows(gu, 0, ni), Int4Rows(gu, ni, 2 * ni)
-        m.gate_up_weight = None
-        m.down_proj = Int4Linear(*w['down_proj'])
 
     @classmethod
     @torch.no_grad()
@@ -562,21 +570,28 @@ class LlamaForCausalLM(LookaheadPreTrainedModel):
             raise ValueError('this model holds int4 weights, which only the int4 GEMM runs: PIA_GEMM=0 / PIA_GEMM_SET '
                              'do not apply')
         b.fp8_out = torch.zeros((b.rows, self.config.hidden_size), dtype=torch.bfloat16, device=b.y.device)
+        n_sm = torch.cuda.get_device_properties(b.y.device).multi_processor_count
+        plans = {'layers': [self._layer_w4_plans(layer, b, n_sm) for layer in self.model.layers]}
+        b.w4_plans = plans
+        return plans
+
+    def _w4_split(self, w, n_sm):
+        """the int4 GEMM's k chunk is 256 wide: _fp8_split's rule over chunks of that size"""
+        return self._fp8_split(torch.empty((w.shape[0], -(-w.shape[1] // 256) * 128), device='meta'), n_sm)
+
+    def _attn_w4_plans(self, layer, b, n_sm):
+        a = layer.self_attn
+        bias = a.qkv_bias.float() if a.qkv_bias is not None else None
+        return {'qkv': a.qkv_w4.gemm(b.y, bias=bias, split_k=self._w4_split(a.qkv_w4, n_sm), out=b.qkv),
+                'o': a.o_proj.gemm(b.attn, split_k=self._w4_split(a.o_proj, n_sm), out=b.fp8_out)}
+
+    def _layer_w4_plans(self, layer, b, n_sm):
+        m = layer.mlp
         if getattr(b, 'act', None) is None or b.act.shape[0] != b.rows:
             b.act = torch.zeros((b.rows, self.config.intermediate_size), dtype=torch.bfloat16, device=b.y.device)
-        n_sm = torch.cuda.get_device_properties(b.y.device).multi_processor_count
-        plans = {'layers': []}
-        for layer in self.model.layers:
-            a, m = layer.self_attn, layer.mlp
-            bias = a.qkv_bias.float() if a.qkv_bias is not None else None
-            # the int4 GEMM's k chunk is 256 wide: _fp8_split's rule over chunks of that size
-            split = lambda w: self._fp8_split(torch.empty((w.shape[0], -(-w.shape[1] // 256) * 128), device='meta'), n_sm)
-            plans['layers'].append({
-                'qkv': a.qkv_w4.gemm(b.y, bias=bias, split_k=split(a.qkv_w4), out=b.qkv),
-                'o': a.o_proj.gemm(b.attn, split_k=split(a.o_proj), out=b.fp8_out),
-                'gate_up_silu': m.gate_up_w4.gemm(b.y, out=b.act).set_silu(),
-                'down': m.down_proj.gemm(b.act, split_k=split(m.down_proj), out=b.fp8_out)})
-        b.w4_plans = plans
+        plans = self._attn_w4_plans(layer, b, n_sm)
+        plans['gate_up_silu'] = m.gate_up_w4.gemm(b.y, out=b.act).set_silu()
+        plans['down'] = m.down_proj.gemm(b.act, split_k=self._w4_split(m.down_proj, n_sm), out=b.fp8_out)
         return plans
 
     def _convert_checkpoint_keys(self, sd):
