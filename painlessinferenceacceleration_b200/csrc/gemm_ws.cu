@@ -1253,7 +1253,6 @@ extern "C" int pia_gemm_plan_create(const void *d_w, int N, int K, const void *d
     cudaError_t e = cudaFuncSetAttribute(k_gemm_ws<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_total(4));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_ws<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_total(8));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_stream<2, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_total<2, 4>());
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_stream<2, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_total<2, 8>());
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gemm_stream<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_total<1, 4>());
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); rc = PIA_ERR_CUDA; }
   }
@@ -1591,8 +1590,6 @@ extern "C" int pia_gemm_run(pia_gemm_plan_t *g, int rows, void *d_out, void *str
     const cudaStream_t st = (cudaStream_t)stream;
     if (g->stream_wg == 1)
       PIA_CUDA_CHECK(launch_kernel(k_gemm_stream<1, 4>, dim3((p.N + 63) / 64), dim3(160), stream_smem_total<1, 4>(), st, g->map_w64, g->map_x, p));
-    else if (g->nstage == 8)
-      PIA_CUDA_CHECK(launch_kernel(k_gemm_stream<2, 8>, dim3((p.N + BMW - 1) / BMW), dim3(NTHREADS), stream_smem_total<2, 8>(), st, g->map_w, g->map_x, p));
     else
       PIA_CUDA_CHECK(launch_kernel(k_gemm_stream<2, 4>, dim3((p.N + BMW - 1) / BMW), dim3(NTHREADS), stream_smem_total<2, 4>(), st, g->map_w, g->map_x, p));
     count_launch();

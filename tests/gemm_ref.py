@@ -1,8 +1,10 @@
 # -*- coding: utf-8 -*-
-"""Plain-torch restatement of the weight-streaming GEMMs (csrc/gemm_ws.cu: k_gemm_ws, k_gemm_sk, k_gemm_fp8) for the
-GEMM tests: the plan rules of pia_gemm_plan_create*, exact-integer operands, an fp64 reference with a scale-aware
-comparator, the one-hot routing probe, an fp32 emulation of the kernels' summation order and the wrong kernels
-(mutations) the checks must reject.  Runs on any device; nothing here needs a GPU."""
+"""Plain-torch restatement of the weight-streaming GEMMs (csrc/gemm_ws.cu: k_gemm_ws, k_gemm_stream, k_gemm_sk,
+k_gemm_fp8, k_gemm_w4) for the GEMM tests: the plan rules of pia_gemm_plan_create* and pia_gemm_run down to the kernel
+instance launched, exact-integer operands (int4: codes, zero points and power-of-two scales whose dequantised weight
+is exact), an fp64 reference with a scale-aware comparator, the one-hot routing probe, an fp32 emulation of the
+kernels' summation order and the wrong kernels (mutations) the checks must reject.  Runs on any device; nothing here
+needs a GPU."""
 from collections import namedtuple
 
 import torch
@@ -16,16 +18,49 @@ def _ceil(a, b):
 
 
 # ------------------------------------------------------------------------------------------------ plan rules
-# kind: 'ws' (k_gemm_ws), 'sk' (k_gemm_sk, stream-K), 'fp8' (k_gemm_fp8).  bk: k per pipeline stage (chunk).
-# cps / n_split: chunks per split and splits; cluster: 0 or the cluster size (the splits of a tile reduce on chip);
-# nstage: the kernel instance; sk_grid: stream-K CTAs.
-Plan = namedtuple('Plan', 'kind N K bk n_chunks cps n_split cluster nstage groups tiles sk_grid')
+# kind: 'ws' (k_gemm_ws), 'stream' (k_gemm_stream), 'sk' (k_gemm_sk, stream-K), 'fp8' (k_gemm_fp8), 'w4' (k_gemm_w4).
+# bk: k per pipeline stage (chunk).  cps / n_split: chunks per split and splits; cluster: 0 or the cluster size (the
+# splits of a tile reduce on chip); nstage: the kernel instance's stage count; sk_grid: stream-K CTAs; wg: consumer
+# warpgroups (64-row slices) per k_gemm_stream tile; tiled: the bf16 weight's HBM layout; group / f16: the int4 scale
+# group (k per scale) and scale dtype.
+Plan = namedtuple('Plan', 'kind N K bk n_chunks cps n_split cluster nstage groups tiles sk_grid wg tiled group f16')
+W4_BK = 256                 # k per k_gemm_w4 stage: 128 bytes of codes per weight row
 
 
-def plan(N, K, split_k=1, tiled=False, fp8=False, groups=1, bias=False, n_sm=132):
-    """what pia_gemm_plan_create / _grouped / _create_fp8 / _grouped_fp8 choose on a device with n_sm SMs; raises
-    ValueError where the library refuses the plan"""
+def _split(n_chunks, split_k, want_cluster):
+    split = min(max(want_cluster or split_k, 1), n_chunks)
+    cps = _ceil(n_chunks, split)
+    n_split = _ceil(n_chunks, cps)
+    if want_cluster and n_split != want_cluster:
+        raise ValueError(f'{n_chunks} chunks are too short for {want_cluster} cluster splits')
+    return cps, n_split
+
+
+def plan(N, K, split_k=1, tiled=False, fp8=False, groups=1, bias=False, n_sm=132, silu=False, w4=False, group=128,
+         f16=False):
+    """what pia_gemm_plan_create / _grouped / _create_fp8 / _grouped_fp8 / _create_w4 / _grouped_w4 (+ set_silu)
+    choose on a device with n_sm SMs, and which kernel pia_gemm_run launches; raises ValueError where the library
+    refuses the plan"""
     want_cluster = -split_k if split_k in (-2, -4, -8) else 0
+    if w4:
+        if N % BMW or K % 128:
+            raise ValueError('the int4 GEMM needs N % 128 == 0 and K % 128 == 0')
+        if group <= 0 or group % 128 or K % group:
+            raise ValueError(f'group size {group}: a multiple of 128 that divides K = {K}')
+        if split_k < 1 and not want_cluster:
+            raise ValueError('int4 plans take split_k >= 1 or a cluster split')
+        if groups > 1 and (split_k != 1 or bias):
+            raise ValueError('a grouped int4 plan has one K split and no bias')
+        n_chunks = _ceil(K, W4_BK)
+        cps, n_split = _split(n_chunks, split_k, want_cluster)
+        if bias and n_split > 1 and not want_cluster:
+            raise ValueError('a bias needs split_k == 1 or a cluster split')
+        if silu and (groups > 1 or n_split > 1 or bias):
+            raise ValueError('the SiLU*up epilogue needs one group, split_k == 1 and no bias')
+        tiles = N // BMW
+        nstage = 4 if tiles * n_split * groups <= n_sm else 2
+        return Plan('w4', N, K, W4_BK, n_chunks, cps, n_split, want_cluster, nstage, groups, tiles, 0, 0, True,
+                    group, bool(f16))
     if fp8:
         if N % BMW or K % 128:
             raise ValueError('the fp8 GEMM needs N % 128 == 0 and K % 128 == 0')
@@ -34,16 +69,13 @@ def plan(N, K, split_k=1, tiled=False, fp8=False, groups=1, bias=False, n_sm=132
         if groups > 1 and split_k != 1:
             raise ValueError('a grouped fp8 plan has one K split')
         n_chunks = K // 128
-        split = min(want_cluster or split_k, n_chunks)
-        cps = _ceil(n_chunks, split)
-        n_split = _ceil(n_chunks, cps)
-        if want_cluster and n_split != want_cluster:
-            raise ValueError(f'K = {K} is too short for {want_cluster} cluster splits')
+        cps, n_split = _split(n_chunks, split_k, want_cluster)
         if bias and n_split > 1 and not want_cluster:
             raise ValueError('a bias needs split_k == 1 or a cluster split')
         tiles = N // BMW
         nstage = 6 if tiles * n_split * groups <= n_sm else 3
-        return Plan('fp8', N, K, 128, n_chunks, cps, n_split, want_cluster, nstage, groups, tiles, 0)
+        return Plan('fp8', N, K, 128, n_chunks, cps, n_split, want_cluster, nstage, groups, tiles, 0, 0, True, 0,
+                    False)
     if K % 64:
         raise ValueError('K must be a multiple of 64')
     n_chunks = K // 64
@@ -51,14 +83,11 @@ def plan(N, K, split_k=1, tiled=False, fp8=False, groups=1, bias=False, n_sm=132
         if N % BMW:
             raise ValueError('grouped GEMM needs N % 128 == 0')
         tiles = N // BMW
-        return Plan('ws', N, K, 64, n_chunks, n_chunks, 1, 0, 8 if tiles * groups <= n_sm else 4, groups, tiles, 0)
+        return Plan('ws', N, K, 64, n_chunks, n_chunks, 1, 0, 8 if tiles * groups <= n_sm else 4, groups, tiles, 0,
+                    0, False, 0, False)
     if split_k < -1 and not want_cluster:
         raise ValueError('cluster split-K supports 2, 4 or 8 CTAs')
-    split = min(max(want_cluster or split_k, 1), n_chunks)
-    cps = _ceil(n_chunks, split)
-    n_split = _ceil(n_chunks, cps)
-    if want_cluster and n_split != want_cluster:
-        raise ValueError(f'K = {K} is too short for {want_cluster} cluster splits')
+    cps, n_split = _split(n_chunks, split_k, want_cluster)
     if tiled and N % BMW:
         raise ValueError('a tiled weight needs N % 128 == 0')
     tiles = _ceil(N, BMW)
@@ -67,8 +96,26 @@ def plan(N, K, split_k=1, tiled=False, fp8=False, groups=1, bias=False, n_sm=132
         if not tiled:
             raise ValueError('stream-K needs the tiled weight layout')
         units = (N // BMW) * n_chunks
-        return Plan('sk', N, K, 64, n_chunks, n_chunks, 1, 0, 8, 1, N // BMW, min(units, n_sm))
-    return Plan('ws', N, K, 64, n_chunks, cps, n_split, want_cluster, nstage, 1, tiles, 0)
+        return Plan('sk', N, K, 64, n_chunks, n_chunks, 1, 0, 8, 1, N // BMW, min(units, n_sm), 0, True, 0, False)
+    if silu and (n_split > 1 or N % BMW):
+        raise ValueError('the SiLU*up epilogue needs split_k == 1 and N % 128 == 0')
+    if n_split == 1 and not want_cluster and not silu:
+        # k_gemm_stream: 64-row tiles while they fit in one wave at 3 CTAs per SM, else 128-row tiles; 4 stages
+        wg = 1 if _ceil(N, 64) <= 3 * n_sm else 2
+        return Plan('stream', N, K, 64, n_chunks, cps, 1, 0, 4, 1, _ceil(N, 64 * wg), 0, wg, bool(tiled), 0, False)
+    return Plan('ws', N, K, 64, n_chunks, cps, n_split, want_cluster, nstage, 1, tiles, 0, 0, bool(tiled), 0, False)
+
+
+def instance(p):
+    """the kernel template instance pia_gemm_run launches for plan p, spelled as in csrc/gemm_ws.cu without spaces
+    and with every template argument given"""
+    if p.kind == 'sk':
+        return 'k_gemm_sk'
+    if p.kind == 'stream':
+        return f'k_gemm_stream<{p.wg},{p.nstage}>'
+    if p.kind == 'w4':
+        return f'k_gemm_w4<{p.nstage},{str(p.f16).lower()},{str(p.groups > 1).lower()}>'
+    return f'k_gemm_{p.kind}<{p.nstage}>'
 
 
 def splits_reported(p):
@@ -157,6 +204,80 @@ def exact_operands(rows, N, K, gen, groups=1, fp8=False, bias=False, device='cpu
     return mv(x), mv(w), mv(scale), mv(b)
 
 
+W4 = namedtuple('W4', 'u s z group')   # int4 weights: codes u [G, N, K], scales s [G, N, K / group], zero points z
+
+
+def dequant_w4(q, mut=None):
+    """the weight k_gemm_w4 multiplies with, bf16 [G, N, K]: W[n, k] = bf16(dtype_s(s[g, n] * (u[n, k] - z[g, n]))),
+    g = the scale group of k's 128-k half; u - z is exact in the scale's dtype, the product rounds once to it.  mut: a
+    key of MUTATIONS that changes which scale a weight takes or how the product rounds."""
+    u, s, z, gs = q
+    G, N, K = u.shape
+    k = torch.arange(K, device=u.device)
+    gi = (k // 128) * 128 // gs
+    if mut == "a half takes its chunk's first group's scale and zero point":
+        gi = (k // W4_BK) * W4_BK // gs
+    if mut == 'rows r and r + 8 swap scales':
+        s = s[:, torch.arange(N, device=u.device) ^ 8]
+    if mut == "a grouped plan reads expert 0's table columns":
+        s, z = s[:1].expand_as(s), z[:1].expand_as(z)
+    d = u.to(s.dtype) - z[:, :, gi].to(s.dtype)
+    if mut == 'the fp16 product is not rounded to fp16 before bf16':
+        return (d.float() * s[:, :, gi].float()).to(torch.bfloat16)
+    return (d * s[:, :, gi]).to(torch.bfloat16)
+
+
+def dense(w):
+    """the bf16 / e4m3 / float weight [G, N, K] a plan multiplies with: int4 codes dequantised"""
+    return dequant_w4(w) if isinstance(w, W4) else w
+
+
+def exact_operands_w4(rows, N, K, group, gen, groups=1, f16=False, bias=False, device='cpu'):
+    """int4 exact-integer operands: x as exact_operands gives it, codes u 0..15, zero points covering 0..16 and
+    power-of-two scales 2^-4 .. 2^-2 that differ between adjacent scale groups and between rows n, n ^ 1 and n ^ 8,
+    so that the dequantised weight is s (u - z) exactly (|W| <= 4 on a 2^-4 grid, in bf16 and fp16 alike) and
+    sum_k |x_k| |W_k| < MASS_LIMIT: every partial sum is exact in fp32 and the output is bf16_rne(exact).  Rows
+    n % 4 < 2 have u >= z.  fp16: rows n % 16 == 5 take the 11-bit scale 2^e (1 + 3 * 2^-10) and u - z in {0, 3}, whose
+    product rounds to fp16 on a tie and then to bf16 on a tie: W = 3 * 2^e exactly, but 3 * 2^e (1 + 2^-6) when the
+    product goes straight to bf16.  Returns (x, W4(u, s, z, group), None, bias)."""
+    x, _, _, _ = exact_operands(rows, N, K, gen, groups=groups)
+    ng = K // group
+    n = torch.arange(N)[:, None]
+    j = torch.arange(ng)[None, :]
+    r16 = torch.randint(0, 3, (groups, N // 16 + 1, 1), generator=gen)[:, n.squeeze(1) // 16]
+    e = -4 + ((n & 1) + 2 * ((n >> 3) & 1) + j + r16) % 3                         # [groups, N, ng]
+    z = torch.randint(0, 17, (groups, N, ng), generator=gen)
+    pos = (torch.arange(N) % 4) < 2
+    z[:, pos] = torch.randint(0, 9, z[:, pos].shape, generator=gen)
+    zn = z[0, ~pos].reshape(-1)
+    zn[:17] = torch.arange(17)                                                    # every zero point appears
+    z[0, ~pos] = zn.view(-1, ng)
+    zk = z.repeat_interleave(group, 2)
+    u = torch.randint(0, 16, (groups, N, K), generator=gen)
+    lo = torch.rand((groups, N, K), generator=gen)
+    u[:, pos] = (zk[:, pos] + (lo[:, pos] * (16 - zk[:, pos])).long()).clamp_max(15)   # u >= z where z <= 15
+    sdt = torch.float16 if f16 else torch.bfloat16
+    s = torch.pow(2.0, e.double())
+    if f16:
+        odd = (torch.arange(N) % 16) == 5
+        s[:, odd] *= 1 + 3 * 2.0 ** -10
+        zo = torch.randint(0, 13, z[:, odd].shape, generator=gen)
+        z[:, odd] = zo
+        u[:, odd] = zo.repeat_interleave(group, 2) + 3 * torch.randint(0, 2, u[:, odd].shape, generator=gen)
+    q = W4(u.to(torch.uint8), s.to(sdt), z.to(torch.uint8), group)
+    assert torch.equal(q.s.double(), s)
+    w = dequant_w4(q).double()
+    assert torch.equal(w * 16, (w * 16).round()) and float(w.abs().max()) <= 4
+    if f16:
+        assert not torch.equal(dequant_w4(q, 'the fp16 product is not rounded to fp16 before bf16').double(), w)
+    for g in range(groups):
+        mass = x[:, g * K:(g + 1) * K].double().abs() @ w[g].abs().t()
+        assert float(mass.max()) < MASS_LIMIT
+    b = torch.randint(-64, 65, (N,), generator=gen).float() if bias else None
+    mv = lambda t: None if t is None else t.to(device)  # noqa: E731
+    return mv(x), W4(*(mv(t) for t in q[:3]), group), None, mv(b)
+
+
 def onehot_x(K, c, rows=TOK, device='cpu'):
     """the routing probe: row t one-hot at k = 64 c + t (rows past K stay zero), so out[t, n] == W[n, 64 c + t]
     exactly; c = 0 .. K / 64 - 1 visits every (n, k) pair once"""
@@ -169,7 +290,8 @@ def onehot_x(K, c, rows=TOK, device='cpu'):
 # ------------------------------------------------------------------------------------------------ reference
 def reference(x, w, scale=None, bias=None):
     """(ref, mass) in fp64 for one group: ref = x @ (w * scale)^T (+ bias), mass = |x| @ |w * scale|^T (+ |bias|).
-    x [rows, K], w [N, K] bf16 / e4m3 / float, scale [N] or None, bias [N] or None"""
+    x [rows, K], w [N, K] bf16 / e4m3 / float (or int4 W4 codes of one group), scale [N] or None, bias [N] or None"""
+    w = dense(w)
     wd = w.double() if w.dtype != torch.float8_e4m3fn else w.float().double()
     if scale is not None:
         wd = wd * scale.double()[:, None]
@@ -241,11 +363,20 @@ MUTATIONS = {
     'last (short) split dropped': lambda p: p.n_split > 1 and not p.cluster,
     'cluster write-out quad tokens swapped': lambda p: p.cluster > 0,
     "adjacent row's fp8 scale": lambda p: p.kind == 'fp8',
-    'bias added per split': lambda p: p.kind == 'fp8' and p.cluster > 0,
+    'bias added per split': lambda p: p.kind in ('fp8', 'w4') and p.cluster > 0,
     'cluster partials rounded to bf16 before the sum': lambda p: p.cluster > 0,
     'round toward zero (__float2bfloat16_rz)': lambda p: p.cluster > 0 or p.n_split == 1,
     'grouped GEMM reads the wrong X column offset': lambda p: p.groups > 1,
+    "a half takes its chunk's first group's scale and zero point": lambda p: p.kind == 'w4' and p.group % W4_BK != 0,
+    'rows r and r + 8 swap scales': lambda p: p.kind == 'w4',
+    'the fp16 product is not rounded to fp16 before bf16': lambda p: p.kind == 'w4' and p.f16,
+    'the half chunk is dropped': lambda p: p.kind == 'w4' and p.K % W4_BK == 128,
+    "a grouped plan reads expert 0's table columns": lambda p: p.kind == 'w4' and p.groups > 1,
+    'a 64-row k_gemm_stream tile reads the other half of its 128-row block':
+        lambda p: p.kind == 'stream' and p.wg == 1 and p.tiled,
 }
+W4_MUTATIONS = {"a half takes its chunk's first group's scale and zero point", 'rows r and r + 8 swap scales',
+                'the fp16 product is not rounded to fp16 before bf16', "a grouped plan reads expert 0's table columns"}
 
 
 def _bf16(v, rz=False):
@@ -266,11 +397,19 @@ def _acc(P, b0, b1, skip=None):
 def emulate(p, x, w, scale=None, bias=None, mut=None):
     """the kernel's arithmetic in torch: each 16-k block product exact, rounded to fp32 and added to an fp32
     accumulator that starts at 0 for every (tile, split) / stream-K segment; fp8: the partial times s[n] in fp32;
-    cluster: partials summed in split order, then + bias, one bf16 rounding; slices: the fp32 partials; stream-K: the
-    owner's segment plus the contributor slots in order.  x [rows, groups * K], w [groups, N, K] (bf16 / e4m3 / float),
-    scale [groups * N], bias [N].  mut: a key of MUTATIONS.  Returns bf16 [rows, N] (or [groups, rows, N]), or fp32
-    slices [n_split, rows, N]."""
+    int4: the dequantised weight, 256-k chunks of which the last is a 128-k half when K % 256 == 128; cluster:
+    partials summed in split order, then + bias, one bf16 rounding; slices: the fp32 partials; stream-K: the owner's
+    segment plus the contributor slots in order; k_gemm_stream: k_gemm_ws's split-1 sums.  x [rows, groups * K], w
+    [groups, N, K] (bf16 / e4m3 / float, or W4 codes), scale [groups * N], bias [N].  mut: a key of MUTATIONS.  Returns
+    bf16 [rows, N] (or [groups, rows, N]), or fp32 slices [n_split, rows, N]."""
     rows, K, N = x.shape[0], p.K, p.N
+    if isinstance(w, W4):
+        w = dequant_w4(w, mut if mut in W4_MUTATIONS else None)
+        if mut == 'the half chunk is dropped':
+            w = w.clone()
+            w[:, :, K - 128:] = 0
+    if mut == 'a 64-row k_gemm_stream tile reads the other half of its 128-row block':
+        w = w[:, torch.arange(N, device=w.device) ^ 64]
     outs = []
     for g in range(p.groups):
         x0 = g * K + (64 if mut == 'grouped GEMM reads the wrong X column offset' else 0)
@@ -293,7 +432,7 @@ def emulate(p, x, w, scale=None, bias=None, mut=None):
                 out[:, t * BMW:(t + 1) * BMW] = acc
             outs.append(_bf16(out, mut == 'round toward zero (__float2bfloat16_rz)'))
             continue
-        parts = [_acc(P, c0 * bpc, c1 * bpc, skip) for c0, c1 in split_ranges(p)]
+        parts = [_acc(P, c0 * bpc, min(c1 * bpc, nb), skip) for c0, c1 in split_ranges(p)]
         if scale is not None:
             sc = scale[g * N:(g + 1) * N].float().to(x.device)
             if mut == "adjacent row's fp8 scale":
@@ -334,11 +473,11 @@ def slice_sum(slices):
 
 def exact_slices(p, x, w, scale=None):
     """the fp32 slices exact-integer operands must produce bit for bit: the exact partial sum of every split's k range
-    (times s[n] for fp8), [n_split, rows, N]"""
+    (times s[n] for fp8; the dequantised weight for int4), [n_split, rows, N]"""
     out = []
     for c0, c1 in split_ranges(p):
-        k0, k1 = c0 * p.bk, c1 * p.bk
-        r, _ = reference(x[:, k0:k1], w[0][:, k0:k1], None if scale is None else scale[:p.N])
+        k0, k1 = c0 * p.bk, min(c1 * p.bk, p.K)
+        r, _ = reference(x[:, k0:k1], dense(w)[0][:, k0:k1], None if scale is None else scale[:p.N])
         out.append(r)
     return torch.stack(out)
 
@@ -348,9 +487,11 @@ def mutation_names(p):
 
 
 def describe(p):
-    """a short path label: kernel, split mode, stage count"""
+    """a short path label: the kernel instance, split mode, layout / groups"""
     if p.kind == 'sk':
         return f'k_gemm_sk units/CTAs={p.tiles * p.n_chunks}/{p.sk_grid}'
+    if p.kind == 'stream':
+        return f'{instance(p)} split1 {"tiled" if p.tiled else "row-major"}'
     mode = f'cluster{p.cluster}' if p.cluster else ('split1' if p.n_split == 1 else f'slices{p.n_split}')
-    name = 'k_gemm_fp8' if p.kind == 'fp8' else 'k_gemm_ws'
-    return f'{name}<{p.nstage}> {mode}' + (f' groups={p.groups}' if p.groups > 1 else '')
+    out = f'{instance(p)} {mode}' + (f' groups={p.groups}' if p.groups > 1 else '')
+    return out + (f' group={p.group}{" fp16" if p.f16 else " bf16"} scales' if p.kind == 'w4' else '')

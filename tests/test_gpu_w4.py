@@ -63,23 +63,31 @@ def _codes(N, K, gs, seed, sdt=torch.bfloat16, sym=False):
 
 
 # (name, N, K, group, bias, split modes): Llama-2-7B, Llama-3-8B, Qwen2-7B (biased qkv), Qwen2.5-0.5B (K = 896 ends in a
-# half chunk)
+# half chunk); Llama-3-8B at group 256 and channel-wise scales (group = K: one scale per row, Qwen2.5-0.5B's qkv with
+# a half chunk under the channel's single group)
 SHAPES = [('llama2_qkv', 12288, 4096, 128, False, (1, -2)), ('llama2_o', 4096, 4096, 128, False, (1, -4, 4)),
           ('llama2_gate_up', 22016, 4096, 128, False, (1,)), ('llama2_down', 4096, 11008, 128, False, (1, -4, 4)),
           ('llama3_qkv', 6144, 4096, 128, False, (1, -2)), ('llama3_gate_up', 28672, 4096, 128, False, (1,)),
           ('llama3_down', 4096, 14336, 128, False, (-4, 8)),
           ('qwen2_qkv', 4608, 3584, 128, True, (1, -4)), ('qwen2_down', 3584, 18944, 128, False, (-4, -8)),
-          ('qwen25_qkv', 1152, 896, 128, True, (1, -2)), ('qwen25_down', 896, 4864, 128, False, (1, -4))]
+          ('qwen25_qkv', 1152, 896, 128, True, (1, -2)), ('qwen25_down', 896, 4864, 128, False, (1, -4)),
+          ('llama3_qkv_g256', 6144, 4096, 256, False, (1, -2)), ('llama3_gate_up_g256', 28672, 4096, 256, False, (1,)),
+          ('llama3_down_g256', 4096, 14336, 256, False, (-4, 8)),
+          ('llama2_down_channel', 4096, 11008, 11008, False, (1, -4, 4)),
+          ('qwen25_qkv_channel', 1152, 896, 896, True, (1, -2))]
 ROWS = (1, 5, 64, 128, 256)
 
 
 @pytest.mark.parametrize('name,N,K,gs,biased,splits', SHAPES)
 def test_w4_gemm_against_fp64(name, N, K, gs, biased, splits):
     """out = bf16(X @ W^T (+ bias)) of the dequantised weight against fp64 with tests/gemm_ref.py's comparator, for
-    1..256 rows and every split mode; two runs bit-identical; rows beyond `rows` untouched"""
-    u, s, z = _codes(N, K, gs, seed=N + K)
-    w = _ops().dequantize_w4(u, s, z, gs).to(DEV)
-    u, s, z = u.to(DEV), s.to(DEV), z.to(DEV)
+    1..256 rows and every split mode; two runs bit-identical; rows beyond `rows` untouched.  The codes are generated on
+    the device (uniform codes, scales around 0.02, zero points 6..10)."""
+    g = torch.Generator(device=DEV).manual_seed(N + K + gs)
+    u = torch.randint(0, 16, (N, K), generator=g, device=DEV, dtype=torch.uint8)
+    s = (0.01 + 0.02 * torch.rand((N, K // gs), generator=g, device=DEV)).to(torch.bfloat16)
+    z = torch.randint(6, 11, (N, K // gs), generator=g, device=DEV, dtype=torch.uint8)
+    w = _ops().dequantize_w4(u, s, z, gs)
     x = torch.randn((256, K), generator=torch.Generator(device=DEV).manual_seed(1), device=DEV).to(torch.bfloat16)
     bias = (torch.randn(N, device=DEV) * 2).to(torch.bfloat16).float() if biased else None
     ref, mass = gemm_ref.reference(x, w, None, bias)
